@@ -8,7 +8,8 @@
 //                   TMA box {32 ch, 16 x, 8 y, 1 n} of the NHWC activation at the
 //                   tap-shifted coordinate (out-of-bounds -> zero fill = zero padding,
 //                   no im2col, no halo staging code) plus one {32 k, N} weight box.
-//   roles       warpgroups 0 / 1: MMAs (M = 64 rows each) and the epilogue of their rows | warp 8: TMA producer
+//   roles       warpgroups 0 / 1: MMAs (M = 64 rows each) and the epilogue of their rows | warpgroup 2: TMA producer
+//               (one elected thread issues the loads; the warpgroup gives its registers to the consumers with setmaxnreg)
 //   pipelines   smem full/empty ring, persistent over tiles: the producer runs ahead into the next tile while the
 //               warpgroups run the epilogue of the current one.
 //   stride 2    TMA element strides {1, 2, 2, 1}: the box spans 32 x 16 pixels, every second one is delivered.
@@ -42,7 +43,11 @@ constexpr int STG_PITCH = 32;                       // floats per staged row; th
                                                     // 128-bit row writes (phase 1) and row-segment reads (phase 2) without padding
 constexpr int EPI_WG_BYTES = 64 * 64 * 4;           // per warpgroup: a 64-row x 64-column accumulator slice, then the four warps' staging areas
 constexpr int BAR_BYTES = 512;
-constexpr int CONSUMER_THREADS = 256, TC_THREADS = CONSUMER_THREADS + 32;
+// warpgroups 0 / 1 consume, warpgroup 2 produces.  A whole producer warpgroup (not one warp) so that it can hand its registers to
+// the consumers with setmaxnreg.  The launch budget is 168 per thread (65536 / 384, in steps of 8): 128 x (2 x 232 + 40) = 384 x 168.
+// 232 holds acc + racc of the split kernel at N = 128 without spills.
+constexpr int CONSUMER_THREADS = 256, TC_THREADS = CONSUMER_THREADS + 128;
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
 struct Params {
   int taps, kw, ph, pw;
@@ -240,9 +245,10 @@ conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   }
   __syncthreads();
 
-  if (warp == CONSUMER_THREADS / 32) {
-    // ===================================================== TMA producer
-    if (elect_one()) {
+  if (warp >= CONSUMER_THREADS / 32) {
+    // ===================================================== TMA producer (one elected thread of the producer warpgroup)
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_THREADS / 32 && elect_one()) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int nt = tile % p.tiles_n; int r = tile / p.tiles_n;
@@ -270,17 +276,19 @@ conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   }
 
   // ===================================================== consumer warpgroups
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wq = warp & 3, gid = lane >> 2, tig = lane & 3;
-  uint8_t* ebuf = epi_base + wg * EPI_WG_BYTES;
-  const uint32_t ebuf_s = smem_u32(ebuf);
+  const uint32_t ebuf_s = smem_u32(epi_base + wg * EPI_WG_BYTES);
   float acc[N / 2];
   float racc[SPLIT ? N / 2 : 1];
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
   int stage = 0; uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int nt = tile % p.tiles_n; int r = tile / p.tiles_n;
     const int tx = r % p.tiles_x; r /= p.tiles_x; const int ty = r % p.tiles_y; const int n = r / p.tiles_y;
+    // (the first MMA of a tile overwrites acc; defining it here ends the previous tile's values, so that they need no registers
+    // through the epilogue)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
     if (SPLIT) {
 #pragma unroll
       for (int i = 0; i < (SPLIT ? N / 2 : 1); ++i) racc[i] = 0.f;
@@ -380,8 +388,8 @@ conv2d_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = wq * 16 + gid + 8 * h;
-          *reinterpret_cast<float2*>(ebuf + row * 256 + ((((col >> 2) ^ (row & 7))) << 4) + (col & 3) * 4) =
-              make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
+          // (32-bit shared addresses: 64-bit generic ones stay live across the column passes and cost registers)
+          sts64(ebuf_s + (uint32_t)(row * 256 + ((((col >> 2) ^ (row & 7))) << 4) + (col & 3) * 4), res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
         }
       }
       wg_sync(1 + wg);

@@ -64,6 +64,11 @@ __device__ __forceinline__ bool elect_one() {
 }
 // named barrier of one 128-thread warpgroup (ids 1.. ; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// per-thread register budget of the executing warpgroup (all of its warps execute it): producers give registers back, consumers take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // sm_90 shared-memory matrix descriptor of a K-major, SWIZZLE_128B operand tile: rows of 128 B, 8-row atoms of 1024 B (SBO).
 // The K offset inside the 128-byte row is applied by advancing the start address (+2 per 32 bytes in the addr >> 4 field).
