@@ -938,7 +938,8 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
         corr_lookup(cx, pyr.view(0), coords1, corr);
       }
       coords_minus_grid(cx, coords1, flow, hx.slice(382, 2));
-      if (it == 0) tap("raft.corr_it0", corr);
+      // (a copy: every later iteration's lookup overwrites `corr`)
+      if (it == 0 && debug_) { TV snap = A.tensor(2 * B, h, w, 324); copy_channels(cx, corr, snap); tap("raft.corr_it0", snap); }
       // BasicMotionEncoder raft/update.py:94-112
       N.conv(u + ".encoder.convc1", corr, cor1, ACT_RELU);
       N.conv(u + ".encoder.convc2", cor1, corflo.slice(0, 192), ACT_RELU);

@@ -317,7 +317,10 @@ class EngineHandle:
         return (out, layers) if per_layer else out
 
     def tap(self, name: str) -> torch.Tensor:
-        """Debug: copy of an intermediate NHWC tensor of the last forward (set_debug(True) first)."""
+        """Debug: copy of an intermediate NHWC tensor of the last forward (set_debug(True) first).
+        Taps are read as float32: every tapped tensor is fp32 in all precision modes (the half-precision chains of modes 3-4 are
+        not tapped).  The per-timestep taps (gimm.splat0, gimm.latent, syn.*) are taken at the first timestep, and the buffers they
+        point into are reused by the following ones: read them after a forward with T = 1."""
         v = View()
         self.lib.check(self.lib.dll.gimmvfi_get_tap(self._h, name.encode(), C.byref(v)), self._h)
         base = self._ws.data_ptr()

@@ -61,10 +61,9 @@ def limits(model):
                 flow4_p9999=5e-2 if tf32 else 1e-2, raft_max=1e-2, repeat=6e-4 if tf32 else 2e-5)
 
 
-@pytest.mark.parametrize("name", ["r_128x160_t0.5", "r_b2_128x192_t0.25_0.75", "r_ds0.5_256x320_t0.5", "r_256x448_t0.5"])
-def test_forward_matches_reference_golden(name, golden_manifest, model):
-    meta = golden_manifest[name]
-    g = load_golden(name)
+def golden_checks(model, meta, g):
+    """Runs `model` on the fixture's case and returns [(what, measured, bar)] for every stored output (the fixture `g` holds the
+    reference's outputs, sub-sampled by g["stride"])."""
     s = int(g["stride"])
     L = limits(model)
     _, out = run_model(model, meta)
@@ -83,9 +82,18 @@ def test_forward_matches_reference_golden(name, golden_manifest, model):
         checks.append(("imgt_pred[%d] |mean diff|" % i, sm, 1e-4))
     rf = out["raft_flow"][..., :: 2 * s, :: 2 * s].cpu()
     checks.append(("raft_flow max", stats(rf, torch.from_numpy(g["raft_flow"]))[0], L["raft_max"]))
+    return checks
+
+
+def report_checks(name, model, checks):
     report = "; ".join("%s %.3e (<= %.1e)%s" % (n, v, lim, "" if v <= lim else " FAIL") for n, v, lim in checks)
     print(name, "mode", model.tensor_cores, report)
     assert all(v <= lim for _, v, lim in checks), report
+
+
+@pytest.mark.parametrize("name", ["r_128x160_t0.5", "r_b2_128x192_t0.25_0.75", "r_ds0.5_256x320_t0.5", "r_256x448_t0.5"])
+def test_forward_matches_reference_golden(name, golden_manifest, model):
+    report_checks(name, model, golden_checks(model, golden_manifest[name], load_golden(name)))
 
 
 def test_forward_matches_oracle_all_outputs(golden_manifest, model, weights0):

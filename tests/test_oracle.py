@@ -46,6 +46,32 @@ def test_oracle_matches_reference_golden(name, golden_manifest, weights0):
     assert np.abs(rf - g["raft_flow"]).max() <= 50 * TOL
 
 
+@pytest.mark.parametrize("name", ["r8_136x200_t0.5", "r8_b2_128x136_t0.25_0.75", "r8_ds0.5_272x400_t0.5"])
+def test_oracle_matches_reference_golden_r8(name, weights0):
+    """Frame sizes that are multiples of 8 but not of 32 (oracle/make_golden_r8.py): RAFT on odd h/8 x w/8 grids, a correlation
+    pyramid that floors odd levels.  Full-resolution fixtures (stride 1)."""
+    import json
+
+    with open(os.path.join(GOLDEN_DIR, "manifest_r8.json")) as f:
+        meta = json.load(f)[name]
+    assert meta["oracle_vs_reference_max_abs"] <= 2e-6
+    g = load_golden(name)
+    s = int(g["stride"])
+    out = run_case(name, meta, weights0)
+    for i in range(len(meta["timesteps"])):
+        a = out["imgt_pred"][i][..., ::s, ::s].numpy()
+        assert a.shape == g["imgt_pred_%d" % i].shape
+        assert np.abs(a - g["imgt_pred_%d" % i]).max() <= TOL
+        f = out["flowt"][i][..., ::s, ::s].numpy()
+        assert f.shape == g["flowt_%d" % i].shape
+        assert np.abs(f - g["flowt_%d" % i]).max() <= 50 * TOL
+        w4 = out["other_pred"][i][0][..., :: 2 * s, :: 2 * s].numpy()
+        assert np.abs(w4 - g["img_warp_4_%d" % i]).max() <= TOL
+        assert np.abs(out["flowt0_pred"][i][1][..., ::s, ::s].numpy() - g["flowt0_4_%d" % i]).max() <= 50 * TOL
+    rf = out["raft_flow"][..., :: 2 * s, :: 2 * s].numpy()
+    assert np.abs(rf - g["raft_flow"]).max() <= 50 * TOL
+
+
 def test_output_contract(golden_manifest, weights0):
     """Keys / shapes of the returned dict (gimmvfi_r.py:398-407), incl. the B=1 flowt squeeze."""
     meta = golden_manifest["r_128x160_t0.5"]
