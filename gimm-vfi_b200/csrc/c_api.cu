@@ -35,6 +35,13 @@ static Problem to_problem(const gimmvfi_problem* p) {
   Problem q; q.B = p->batch; q.Hf = p->height; q.Wf = p->width; q.T = p->timesteps; q.ds = p->ds_factor; q.Hc = p->coord_height; q.Wc = p->coord_width;
   return q;
 }
+static IO to_io(const gimmvfi_io* io) {
+  IO q;
+  q.img_xs = io->img_xs; q.coords = io->coords; q.t = io->t; q.imgt_pred = io->imgt_pred; q.img_warp_4 = io->img_warp_4;
+  q.flowt0_1 = io->flowt0_1; q.flowt1_1 = io->flowt1_1; q.flowt0_4 = io->flowt0_4; q.flowt1_4 = io->flowt1_4;
+  q.raft_flow = io->raft_flow; q.nflow = io->nflow; q.ninrflow = io->ninrflow; q.flowt = io->flowt;
+  return q;
+}
 
 extern "C" {
 
@@ -55,22 +62,9 @@ int gimmvfi_plan(gimmvfi_engine* e, const gimmvfi_problem* p, size_t* workspace_
 
 int gimmvfi_forward(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_io* io, void* workspace, size_t workspace_bytes,
                     void* cuda_stream) {
-  GV_TRY(e, {
-    IO q;
-    q.img_xs = io->img_xs; q.coords = io->coords; q.t = io->t; q.imgt_pred = io->imgt_pred; q.img_warp_4 = io->img_warp_4;
-    q.flowt0_1 = io->flowt0_1; q.flowt1_1 = io->flowt1_1; q.flowt0_4 = io->flowt0_4; q.flowt1_4 = io->flowt1_4;
-    q.raft_flow = io->raft_flow; q.nflow = io->nflow; q.ninrflow = io->ninrflow; q.flowt = io->flowt;
-    e->eng.forward(to_problem(p), q, workspace, workspace_bytes, (gvStream_t)cuda_stream);
-  })
+  GV_TRY(e, { e->eng.forward(to_problem(p), to_io(io), workspace, workspace_bytes, (gvStream_t)cuda_stream); })
 }
 
-static IO to_io(const gimmvfi_io* io) {
-  IO q;
-  q.img_xs = io->img_xs; q.coords = io->coords; q.t = io->t; q.imgt_pred = io->imgt_pred; q.img_warp_4 = io->img_warp_4;
-  q.flowt0_1 = io->flowt0_1; q.flowt1_1 = io->flowt1_1; q.flowt0_4 = io->flowt0_4; q.flowt1_4 = io->flowt1_4;
-  q.raft_flow = io->raft_flow; q.nflow = io->nflow; q.ninrflow = io->ninrflow; q.flowt = io->flowt;
-  return q;
-}
 int gimmvfi_finalize_weights_synthesis(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_synthesis(); }) }
 int gimmvfi_finalize_weights_f(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_f(); }) }
 int gimmvfi_set_flowformer_iters(gimmvfi_engine* e, int iters) { GV_TRY(e, { if (iters < 1) throw std::runtime_error("iters must be >= 1"); e->eng.ff_iters = iters; }) }
@@ -396,7 +390,7 @@ int gimmvfi_op_conv2d_halo(const gimmvfi_view* in0, const void* w_tc_h, const fl
 }
 int gimmvfi_op_hyponet(gimmvfi_engine* e, const gimmvfi_view* latent, const float* coords, const gimmvfi_view* out, int fp32_class, void* stream) {
   GV_TRY(e, {
-    if (!e->eng.finalized() || !e->eng.hyponet_blob(fp32_class != 0)) throw std::runtime_error("hyponet: finalize_weights() first");
+    e->eng.need(Engine::Entry::Gimm);
     Ctx cx = op_ctx(stream);
     if (out->h != latent->h || out->w != latent->w) {   // another grid size: the latent is resized to it inside the fp32-class kernel
       if (!fp32_class) throw std::runtime_error("hyponet: an output grid of another size than the latent needs fp32_class = 1");

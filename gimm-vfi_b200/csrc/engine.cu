@@ -144,11 +144,7 @@ Engine::Engine(int device) : device_(device) {
   if (const char* kn = getenv("GIMMVFI_RAFT_CORR_DIRECT_GB")) raft_direct_auto_bytes_ = atof(kn) * 1e9;
 }
 
-Engine::~Engine() {
-  clear_graphs();
-  DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-}
+Engine::~Engine() { drop_weights(); }
 
 void Engine::load_weight(const std::string& key, const float* host, const int64_t* shape, int ndim) {
   HostTensor t;
@@ -156,7 +152,51 @@ void Engine::load_weight(const std::string& key, const float* host, const int64_
   for (int i = 0; i < ndim; ++i) { t.shape.push_back(shape[i]); n *= shape[i]; }
   t.data.assign(host, host + n);
   raw_[key] = std::move(t);
-  finalized_ = false;
+  held_ = Weights::None;
+}
+
+// Frees the device weights, with every pointer into them, and the graphs recorded on them.  A frame cache stored under the old
+// weights must not be loaded again.
+void Engine::drop_weights() {
+  DeviceGuard dg(device_);
+  for (void* p : dev_allocs_) dev_free(p);
+  dev_allocs_.clear(); conv_.clear(); vec_.clear();
+  fc_valid_.clear(); ++weights_version_; clear_graphs();
+  held_ = Weights::None;
+  hypo_blob_ = hypo_blob3_ = nullptr;
+  g9_ = alpha_fe_ = alpha_v_ = nullptr;
+}
+
+void Engine::need(Entry e) const {
+  using W = Weights;
+  auto mask = [](std::initializer_list<W> ws) { unsigned m = 0; for (W w : ws) m |= 1u << (int)w; return m; };
+  // per Entry: the weights a refusal names as missing, and the weight sets that serve the entry point
+  struct EntryRule { const char* needs; unsigned served; };
+  static const EntryRule kEntries[] = {
+      {"GIMM-VFI-R or GIMM-VFI-F", mask({W::R, W::F})},                 // plan, forward
+      {"synthesis", mask({W::R, W::F, W::Synthesis})},                  // plan_from_flow, forward_from_flow
+      {"GIMM", mask({W::R, W::F, W::Synthesis, W::Gimm})},              // plan_gimm, forward_gimm, gimmvfi_op_hyponet
+      {"RAFT", mask({W::R, W::Raft})},                                  // plan_raft, forward_raft
+      {"FlowFormer", mask({W::F, W::FlowFormer})},                      // plan_flowformer, forward_flowformer
+      {"LPIPS", mask({W::Lpips})},                                      // plan_lpips, forward_lpips
+  };
+  // per Weights after None: the set's name, the call that loads it and the entry point it is loaded for
+  struct HeldName { const char* name; const char* finalize; const char* use; };
+  static const HeldName kHeld[] = {
+      {"GIMM-VFI-R", "finalize_weights", "forward"},
+      {"GIMM-VFI-F", "finalize_weights_f", "forward"},
+      {"synthesis", "finalize_weights_synthesis", "forward_from_flow"},
+      {"GIMM", "finalize_weights_gimm", "forward_gimm"},
+      {"RAFT", "finalize_weights_raft", "forward_raft"},
+      {"FlowFormer", "finalize_weights_flowformer", "forward_flowformer"},
+      {"LPIPS", "finalize_weights_lpips", "forward_lpips"},
+  };
+  const EntryRule& r = kEntries[(int)e];
+  if (r.served >> (int)held_ & 1u) return;
+  const std::string msg = std::string("gimmvfi: no ") + r.needs + " weights were loaded";
+  if (held_ == W::None) throw std::runtime_error(msg + " (finalize_weights* has not been called)");
+  const HeldName& h = kHeld[(int)held_ - 1];
+  throw std::runtime_error(msg + ": this engine holds " + h.name + " weights only (" + h.finalize + "); use " + h.use);
 }
 
 const HostTensor& Engine::raw(const std::string& key) const {
@@ -341,15 +381,13 @@ void Engine::pack_xpacked(const std::string& name, int ldp) {
 
 void Engine::finalize_weights() {
   DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();   // a frame cache stored under the old weights must not be loaded again
+  drop_weights();
   finalize_raft();
   // --- feature projections (gimmvfi_r.py:51-53)
   pack_conv("amt_last_cproj"); pack_conv("amt_second_last_cproj"); pack_conv("amt_fproj");
   finalize_decoders();
   finalize_gimm_part();
-  finalized_ = true; gimm_only_ = false; synth_only_ = false; ff_ = false; lpips_ = false; ff_only_ = false; raft_only_ = false;
+  held_ = Weights::R;
 }
 
 // RAFT's parameters (raft/raft.py:62-70) under flow_estimator.: shared by GIMM-VFI-R and the RAFT module alone
@@ -408,22 +446,23 @@ void Engine::finalize_raft() {
   pack_xpacked(u + ".encoder.convf1", 4);
 }
 
-// The RAFT module alone (the reference's initialize_RAFT(), raft/__init__.py:7-24): its state_dict keys, moved under GIMM-VFI-R's
-// "flow_estimator." prefix (replacing what an earlier load left there), so reloading one engine with other weights takes the new ones.
-void Engine::finalize_weights_raft() {
-  DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();
-  finalized_ = false;
-  const std::string fe = "flow_estimator.";
+// A flow estimator loaded on its own: the keys under its children's prefixes are moved under GIMM-VFI's "flow_estimator." prefix
+// (replacing what an earlier load left there), so reloading one engine with other weights takes the new ones.
+void Engine::prefix_flow_estimator(std::initializer_list<const char*> children) {
   std::vector<std::string> bare;
   for (const auto& kv : raw_)
-    for (const char* top : {"fnet.", "cnet.", "update_block."})   // the module's three children (raft.py:62-70)
+    for (const char* top : children)
       if (kv.first.compare(0, std::strlen(top), top) == 0) bare.push_back(kv.first);
-  for (const std::string& k : bare) { raw_[fe + k] = std::move(raw_[k]); raw_.erase(k); }
+  for (const std::string& k : bare) { raw_["flow_estimator." + k] = std::move(raw_[k]); raw_.erase(k); }
+}
+
+// The RAFT module alone (the reference's initialize_RAFT(), raft/__init__.py:7-24)
+void Engine::finalize_weights_raft() {
+  DeviceGuard dg(device_);
+  drop_weights();
+  prefix_flow_estimator({"fnet.", "cnet.", "update_block."});   // the module's three children (raft.py:62-70)
   finalize_raft();
-  finalized_ = true; gimm_only_ = false; synth_only_ = false; ff_ = false; lpips_ = false; ff_only_ = false; raft_only_ = true;
+  held_ = Weights::Raft;
 }
 
 // AMT decoders / update blocks / combine block (fi_components.py:229-305): shared by GIMM-VFI-R and -F
@@ -466,39 +505,30 @@ void Engine::finalize_decoders() {
 // external flow estimator (forward_from_flow); there are no feature projections in F (twins features are used as they are)
 void Engine::finalize_weights_synthesis() {
   DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();
+  drop_weights();
   finalize_decoders();
   finalize_gimm_part();
-  finalized_ = true; gimm_only_ = false; synth_only_ = true; ff_ = false; lpips_ = false; ff_only_ = false; raft_only_ = false;
+  held_ = Weights::Synthesis;
 }
 
 // GIMM-VFI-F complete (gimmvfi_f.py:27-111): the synthesis half + the native FlowFormer estimator (flowformer.cu)
 void Engine::finalize_weights_f() {
-  finalize_weights_synthesis();
   DeviceGuard dg(device_);
+  drop_weights();
+  finalize_decoders();
+  finalize_gimm_part();
   finalize_flowformer();
-  synth_only_ = false; ff_ = true;
+  held_ = Weights::F;
 }
 
 // The FlowFormer module alone (the reference's initialize_Flowformer(), flowformer/__init__.py): its state_dict keys, with or without
-// GIMM-VFI-F's "flow_estimator." prefix.  Unprefixed keys loaded since the last finalize are moved to the prefixed names (replacing what an
-// earlier load left there), so reloading one engine with other weights takes the new ones.
+// GIMM-VFI-F's "flow_estimator." prefix.
 void Engine::finalize_weights_flowformer() {
   DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();
-  finalized_ = false;
-  const std::string fe = "flow_estimator.";
-  std::vector<std::string> bare;
-  for (const auto& kv : raw_)
-    for (const char* top : {"memory_encoder.", "memory_decoder.", "context_encoder."})   // the module's three children (transformer.py:29-39)
-      if (kv.first.compare(0, std::strlen(top), top) == 0) bare.push_back(kv.first);
-  for (const std::string& k : bare) { raw_[fe + k] = std::move(raw_[k]); raw_.erase(k); }
+  drop_weights();
+  prefix_flow_estimator({"memory_encoder.", "memory_decoder.", "context_encoder."});   // the module's three children (transformer.py:29-39)
   finalize_flowformer();
-  finalized_ = true; gimm_only_ = false; synth_only_ = false; ff_ = false; lpips_ = false; ff_only_ = true; raft_only_ = false;
+  held_ = Weights::FlowFormer;
 }
 
 void Engine::tap_copy(Ctx& cx, const std::string& name, const TV& tv) {
@@ -609,11 +639,9 @@ void Engine::finalize_gimm_part() {
 // standalone GIMM checkpoint (SURVEY 8(f) row 4): only the keys of gimm.py's module tree are present
 void Engine::finalize_weights_gimm() {
   DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();
+  drop_weights();
   finalize_gimm_part();
-  finalized_ = true; gimm_only_ = true; ff_ = false; lpips_ = false; ff_only_ = false; raft_only_ = false;
+  held_ = Weights::Gimm;
 }
 
 
@@ -1072,7 +1100,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       nchw_to_nhwc(cx, fin->feat8[j], (int64_t)256 * h * w, (int64_t)h * w, feat8.batch(j * B, B), 1.f, 0.f);
       nchw_to_nhwc(cx, fin->fnet[j], (int64_t)256 * h * w, (int64_t)h * w, fproj.batch(j * B, B), 1.f, 0.f);
     }
-  } else if (ff_) {
+  } else if (is_f()) {
     // GIMM-VFI-F: the native FlowFormer estimator fills the same four products (gimmvfi_f.py:114-138); F has no feature projections
     std::vector<int> src(2 * B), tgt(2 * B);   // frames [I0 ; I1]: pairs (b, B + b), then (B + b, b), one reference call per direction
     for (int s = 0; s < 2 * B; ++s) { src[s] = s; tgt[s] = s < B ? s + B : s - B; }
@@ -1124,7 +1152,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   // Everything downstream of RAFT tolerates TF32 operands (DESIGN.md precision plan).
   cx.tc = tc_mode_ >= 1; cx.tc_split = false;
   // ------------------------------------------------------------ bidirectional volume on projected features
-  if (!fin && !ff_) N.conv("amt_fproj", fmap, fproj);
+  if (!fin && !is_f()) N.conv("amt_fproj", fmap, fproj);
   // the bidirectional volume only feeds TF32 layers (AMT update blocks) -> plain TF32 is at their input precision
   // Few interpolated frames per pair (T <= corr_direct_max_t_): no volume at all - the lookup computes the dot products its window needs
   // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.
@@ -1474,22 +1502,16 @@ void Engine::run_gimm(Ctx& cx, const Problem& P, const GimmIO& io) {
   }
 }
 
-size_t Engine::plan_gimm(const Problem& p) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
+// A workspace plan: `run` is the forward's run_* on a dry context (nothing launched or touched), under the current debug setting
+size_t Engine::dry_run(const std::function<void(Ctx&)>& run) {
   Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  GimmIO io; float* fake = reinterpret_cast<float*>(size_t(64));
-  io.xs = io.ori_flow = io.coords = io.t = fake; io.out = fake;
-  const bool dbg = debug_; debug_ = false;
-  run_gimm(cx, p, io);
-  debug_ = dbg; taps_.clear();
+  run(cx);
+  taps_.clear();
   return cx.arena.peak + 256;
 }
 
-void Engine::forward_gimm(const Problem& p, const GimmIO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
-  if (!io.xs || !io.ori_flow || !io.coords || !io.t || !io.out) throw std::runtime_error("gimm: xs, ori_flow, coords, t and out are required");
+// A forward: `run` launches on the caller's stream, with the workspace as its arena
+void Engine::launch(void* workspace, size_t workspace_bytes, gvStream_t stream, const std::function<void(Ctx&)>& run) {
   DeviceGuard dg(device_);
   Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
   prof_.reset();
@@ -1498,8 +1520,24 @@ void Engine::forward_gimm(const Problem& p, const GimmIO& io, void* workspace, s
   cx.arena.base = reinterpret_cast<char*>(base);
   cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
   taps_.clear();
-  run_gimm(cx, p, io);
+  run(cx);
   launches_ = cx.launches;
+}
+
+// the caller pointers of a dry run: never dereferenced, but optional outputs must be "present"
+static float* const kFake = reinterpret_cast<float*>(size_t(64));
+
+size_t Engine::plan_gimm(const Problem& p) {
+  need(Entry::Gimm);
+  GimmIO io;
+  io.xs = io.ori_flow = io.coords = io.t = kFake; io.out = kFake;
+  return dry_run([&](Ctx& cx) { run_gimm(cx, p, io); });
+}
+
+void Engine::forward_gimm(const Problem& p, const GimmIO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
+  need(Entry::Gimm);
+  if (!io.xs || !io.ori_flow || !io.coords || !io.t || !io.out) throw std::runtime_error("gimm: xs, ori_flow, coords, t and out are required");
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run_gimm(cx, p, io); });
 }
 
 size_t Engine::frame_cache_bytes(const Problem& p) {
@@ -1507,54 +1545,33 @@ size_t Engine::frame_cache_bytes(const Problem& p) {
   return ((size_t)p.B * h * w * 256 * 3 + (size_t)p.B * H4 * W4 * 128) * sizeof(float);
 }
 
+static IO fake_io() {
+  IO io;
+  io.img_xs = io.coords = io.t = kFake;
+  io.imgt_pred = io.img_warp_4 = io.flowt0_1 = io.flowt1_1 = io.flowt0_4 = io.flowt1_4 = io.raft_flow = io.nflow = io.ninrflow = io.flowt = kFake;
+  return io;
+}
+
 size_t Engine::plan_from_flow(const Problem& p) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights*() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
-  if (gimm_only_) throw std::runtime_error("gimmvfi: only GIMM's weights were loaded");
-  Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  IO io; float* fake = reinterpret_cast<float*>(size_t(64));
-  io.img_xs = io.coords = io.t = fake;
-  io.imgt_pred = io.img_warp_4 = io.flowt0_1 = io.flowt1_1 = io.flowt0_4 = io.flowt1_4 = io.raft_flow = io.nflow = io.ninrflow = io.flowt = fake;
-  FlowInputs fin; fin.flows = fake;
-  for (int j = 0; j < 2; ++j) fin.feat4[j] = fin.feat8[j] = fin.fnet[j] = fake;
-  run(cx, p, io, &fin);
-  taps_.clear();
-  return cx.arena.peak + 256;
+  need(Entry::FromFlow);
+  const IO io = fake_io();
+  FlowInputs fin; fin.flows = kFake;
+  for (int j = 0; j < 2; ++j) fin.feat4[j] = fin.feat8[j] = fin.fnet[j] = kFake;
+  return dry_run([&](Ctx& cx) { run(cx, p, io, &fin); });
 }
 
 void Engine::forward_from_flow(const Problem& p, const IO& io, const FlowInputs& fin, void* workspace, size_t workspace_bytes, gvStream_t stream) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights*() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
-  if (gimm_only_) throw std::runtime_error("gimmvfi: only GIMM's weights were loaded (finalize_weights_gimm)");
+  need(Entry::FromFlow);
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: img_xs, coords, t and imgt_pred are required");
   if (!fin.flows || !fin.feat4[0] || !fin.feat4[1] || !fin.feat8[0] || !fin.feat8[1] || !fin.fnet[0] || !fin.fnet[1])
     throw std::runtime_error("gimmvfi: forward_from_flow needs flows, feat4[2], feat8[2] and fnet[2]");
-  DeviceGuard dg(device_);
-  Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
-  prof_.reset();
-  cx.prof = profile_ ? &prof_ : nullptr;
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255);
-  cx.arena.base = reinterpret_cast<char*>(base);
-  cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
-  taps_.clear();
-  run(cx, p, io, &fin);
-  launches_ = cx.launches;
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, &fin); });
 }
 
 size_t Engine::plan(const Problem& p) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
-  if (synth_only_) throw std::runtime_error("gimmvfi: no flow estimator weights were loaded (finalize_weights_synthesis); use plan_from_flow");
-  Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  IO io;  // null pointers; dry run never dereferences them, but optional outputs must be "present"
-  float* fake = reinterpret_cast<float*>(size_t(64));
-  io.img_xs = io.coords = io.t = fake;
-  io.imgt_pred = io.img_warp_4 = io.flowt0_1 = io.flowt1_1 = io.flowt0_4 = io.flowt1_4 = io.raft_flow = io.nflow = io.ninrflow = io.flowt = fake;
-  bool dbg = debug_;
-  run(cx, p, io);
-  debug_ = dbg;
-  taps_.clear();
-  return cx.arena.peak + 256;
+  need(Entry::Interpolate);
+  const IO io = fake_io();
+  return dry_run([&](Ctx& cx) { run(cx, p, io); });
 }
 
 void Engine::clear_graphs() {
@@ -1566,63 +1583,53 @@ void Engine::clear_graphs() {
 }
 
 void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
-  if (!finalized_) throw std::runtime_error("gimmvfi: finalize_weights() has not been called");
-  refuse_lpips(); refuse_ff_only(); refuse_raft_only();
-  if (gimm_only_) throw std::runtime_error("gimmvfi: only GIMM's weights were loaded (finalize_weights_gimm); use gimm_forward");
-  if (synth_only_) throw std::runtime_error("gimmvfi: no flow estimator weights were loaded (finalize_weights_synthesis); use forward_from_flow");
+  need(Entry::Interpolate);
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: img_xs, coords, t and imgt_pred are required");
-  DeviceGuard dg(device_);
-  Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
-  prof_.reset();
-  cx.prof = profile_ ? &prof_ : nullptr;
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255);
-  cx.arena.base = reinterpret_cast<char*>(base);
-  cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
-  taps_.clear();
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) {
 #ifndef GV_HOSTSIM
-  // (the legacy default stream - handles 0 / 1 / 2 - cannot be captured: such callers run eagerly)
-  if (use_graph_ && !profile_ && !debug_ && fc_ == nullptr && reinterpret_cast<uintptr_t>(stream) > 2) {
-    // everything a recorded launch sequence depends on: problem, every caller pointer, the workspace, the arithmetic mode, the weights
-    std::vector<uint64_t> key = {(uint64_t)p.B, (uint64_t)p.Hf, (uint64_t)p.Wf, (uint64_t)p.T, (uint64_t)p.Hc, (uint64_t)p.Wc, 0, (uint64_t)tc_mode_, (uint64_t)precise_,
-                                 (uint64_t)hypo_fast_, (uint64_t)(raft_direct_ + 2), (uint64_t)corr_direct_max_t_, (uint64_t)gru_hoist_, (uint64_t)weights_version_, (uint64_t)raft_iters, (uint64_t)workspace, (uint64_t)workspace_bytes, (uint64_t)(uintptr_t)stream};
-    std::memcpy(&key[6], &p.ds, sizeof(float));
-    const void* ptrs[] = {io.img_xs, io.coords, io.t, io.imgt_pred, io.img_warp_4, io.flowt0_1, io.flowt1_1, io.flowt0_4, io.flowt1_4, io.raft_flow, io.nflow, io.ninrflow, io.flowt};
-    for (const void* q : ptrs) key.push_back((uint64_t)(uintptr_t)q);
-    GraphEntry* hit = nullptr;
-    for (GraphEntry& g : graphs_) if (g.key == key) { hit = &g; break; }
-    if (hit && hit->exec) {
-      cuda_ok(cudaGraphLaunch((cudaGraphExec_t)hit->exec, stream), "cudaGraphLaunch");
-      launches_ = hit->launches; ++graph_replays_;
-      return;
-    }
-    if (hit && hit->seen >= 1) {   // second sighting: record.  (The first call ran eagerly: lazy one-time host work - function attributes - is done.)
-      cudaGraph_t graph = nullptr;
-      cuda_ok(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCapture");
-      try {
-        run(cx, p, io);
-      } catch (...) {
-        cudaStreamEndCapture(stream, &graph);
-        if (graph) cudaGraphDestroy(graph);
-        throw;
+    // (the legacy default stream - handles 0 / 1 / 2 - cannot be captured: such callers run eagerly)
+    if (use_graph_ && !profile_ && !debug_ && fc_ == nullptr && reinterpret_cast<uintptr_t>(stream) > 2) {
+      // everything a recorded launch sequence depends on: problem, every caller pointer, the workspace, the arithmetic mode, the weights
+      std::vector<uint64_t> key = {(uint64_t)p.B, (uint64_t)p.Hf, (uint64_t)p.Wf, (uint64_t)p.T, (uint64_t)p.Hc, (uint64_t)p.Wc, 0, (uint64_t)tc_mode_, (uint64_t)precise_,
+                                   (uint64_t)hypo_fast_, (uint64_t)(raft_direct_ + 2), (uint64_t)corr_direct_max_t_, (uint64_t)gru_hoist_, (uint64_t)weights_version_, (uint64_t)raft_iters, (uint64_t)workspace, (uint64_t)workspace_bytes, (uint64_t)(uintptr_t)stream};
+      std::memcpy(&key[6], &p.ds, sizeof(float));
+      const void* ptrs[] = {io.img_xs, io.coords, io.t, io.imgt_pred, io.img_warp_4, io.flowt0_1, io.flowt1_1, io.flowt0_4, io.flowt1_4, io.raft_flow, io.nflow, io.ninrflow, io.flowt};
+      for (const void* q : ptrs) key.push_back((uint64_t)(uintptr_t)q);
+      GraphEntry* hit = nullptr;
+      for (GraphEntry& g : graphs_) if (g.key == key) { hit = &g; break; }
+      if (hit && hit->exec) {
+        cuda_ok(cudaGraphLaunch((cudaGraphExec_t)hit->exec, stream), "cudaGraphLaunch");
+        cx.launches = hit->launches; ++graph_replays_;
+        return;
       }
-      cuda_ok(cudaStreamEndCapture(stream, &graph), "cudaStreamEndCapture");
-      cudaGraphExec_t exec = nullptr;
-      cuda_ok(cudaGraphInstantiate(&exec, graph, 0), "cudaGraphInstantiate");
-      cudaGraphDestroy(graph);
-      hit->exec = exec; hit->launches = cx.launches;
-      cuda_ok(cudaGraphLaunch(exec, stream), "cudaGraphLaunch");
-      launches_ = cx.launches; ++graph_replays_;
-      return;
+      if (hit && hit->seen >= 1) {   // second sighting: record.  (The first call ran eagerly: lazy one-time host work - function attributes - is done.)
+        cudaGraph_t graph = nullptr;
+        cuda_ok(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCapture");
+        try {
+          run(cx, p, io);
+        } catch (...) {
+          cudaStreamEndCapture(stream, &graph);
+          if (graph) cudaGraphDestroy(graph);
+          throw;
+        }
+        cuda_ok(cudaStreamEndCapture(stream, &graph), "cudaStreamEndCapture");
+        cudaGraphExec_t exec = nullptr;
+        cuda_ok(cudaGraphInstantiate(&exec, graph, 0), "cudaGraphInstantiate");
+        cudaGraphDestroy(graph);
+        hit->exec = exec; hit->launches = cx.launches;
+        cuda_ok(cudaGraphLaunch(exec, stream), "cudaGraphLaunch");
+        ++graph_replays_;
+        return;
+      }
+      if (!hit) {
+        if (graphs_.size() >= 8) { if (graphs_.front().exec) cudaGraphExecDestroy((cudaGraphExec_t)graphs_.front().exec); graphs_.erase(graphs_.begin()); }
+        GraphEntry g; g.key = key; g.seen = 1;
+        graphs_.push_back(g);
+      }
     }
-    if (!hit) {
-      if (graphs_.size() >= 8) { if (graphs_.front().exec) cudaGraphExecDestroy((cudaGraphExec_t)graphs_.front().exec); graphs_.erase(graphs_.begin()); }
-      GraphEntry g; g.key = key; g.seen = 1;
-      graphs_.push_back(g);
-    }
-  }
 #endif
-  run(cx, p, io);
-  launches_ = cx.launches;
+    run(cx, p, io);
+  });
 }
 
 // ---------------------------------------------------------------------------
@@ -1631,7 +1638,6 @@ void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t wor
 // ---------------------------------------------------------------------------
 void Engine::run_flowformer_pairs(Ctx& cx, const float* frames, int F, int H, int W, const std::vector<int>& src, const std::vector<int>& tgt,
                                   int per_call, int iters, bool gather, float* flow_up, float* flow_low) {
-  if (!finalized_ || !(ff_ || ff_only_)) throw std::runtime_error("gimmvfi: no FlowFormer weights were loaded (finalize_weights_flowformer / finalize_weights_f)");
   if (F < 1 || H < 32 || W < 32) throw std::runtime_error("flowformer: at least one frame of at least 32 x 32 pixels is required");
   if (H % 32 || W % 32) throw std::runtime_error("gimmvfi: FlowFormer needs a network resolution that is a multiple of 32 (Twins-SVT sub-sampling)");
   if (iters < 1) throw std::runtime_error("flowformer: iters must be >= 1");
@@ -1648,6 +1654,7 @@ void Engine::run_flowformer_pairs(Ctx& cx, const float* frames, int F, int H, in
 }
 
 size_t Engine::plan_flowformer(int n_frames, int h, int w, int n_pairs) {
+  need(Entry::FlowFormer);
   if (n_pairs < 1) throw std::runtime_error("flowformer: at least one pair is required");
   if (n_frames < 1) throw std::runtime_error("flowformer: at least one frame is required");
   // the most memory any pair list of this size can take: min(F, P) distinct sources and the context gathered into pair order.  This bound
@@ -1655,16 +1662,12 @@ size_t Engine::plan_flowformer(int n_frames, int h, int w, int n_pairs) {
   // per_call, and the gathering path only adds buffers: a change that breaks either must change this plan too.
   std::vector<int> src(n_pairs), tgt(n_pairs);
   for (int s = 0; s < n_pairs; ++s) { src[s] = s % n_frames; tgt[s] = (s + 1) % n_frames; }
-  Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  float* fake = reinterpret_cast<float*>(size_t(64));
-  const bool dbg = debug_; debug_ = false;
-  run_flowformer_pairs(cx, fake, n_frames, h, w, src, tgt, 1, 1, true, fake, fake);
-  debug_ = dbg; taps_.clear();
-  return cx.arena.peak + 256;
+  return dry_run([&](Ctx& cx) { run_flowformer_pairs(cx, kFake, n_frames, h, w, src, tgt, 1, 1, true, kFake, kFake); });
 }
 
 void Engine::forward_flowformer(const float* frames, int n_frames, int h, int w, const int32_t* pairs, int n_pairs, int pairs_per_call, int iters,
                                 float* flow_up, float* flow_low, void* workspace, size_t workspace_bytes, gvStream_t stream) {
+  need(Entry::FlowFormer);
   if (!frames || !pairs || !flow_up) throw std::runtime_error("flowformer: frames, pairs and flow_up are required");
   if (n_pairs < 1) throw std::runtime_error("flowformer: at least one pair is required");
   if (pairs_per_call < 1 || n_pairs % pairs_per_call) throw std::runtime_error("flowformer: n_pairs must be a multiple of pairs_per_call (>= 1)");
@@ -1676,16 +1679,8 @@ void Engine::forward_flowformer(const float* frames, int n_frames, int h, int w,
       throw std::runtime_error("flowformer: pair " + std::to_string(s) + " = (" + std::to_string(src[s]) + ", " + std::to_string(tgt[s]) +
                                ") indexes outside the " + std::to_string(n_frames) + " frames");
   }
-  DeviceGuard dg(device_);
-  Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
-  prof_.reset();
-  cx.prof = profile_ ? &prof_ : nullptr;
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255);
-  cx.arena.base = reinterpret_cast<char*>(base);
-  cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
-  taps_.clear();
-  run_flowformer_pairs(cx, frames, n_frames, h, w, src, tgt, pairs_per_call, iters ? iters : ff_iters, false, flow_up, flow_low);
-  launches_ = cx.launches;
+  launch(workspace, workspace_bytes, stream,
+         [&](Ctx& cx) { run_flowformer_pairs(cx, frames, n_frames, h, w, src, tgt, pairs_per_call, iters ? iters : ff_iters, false, flow_up, flow_low); });
 }
 
 // ---------------------------------------------------------------------------
@@ -1694,7 +1689,6 @@ void Engine::forward_flowformer(const float* frames, int n_frames, int h, int w,
 // ---------------------------------------------------------------------------
 void Engine::run_raft_pairs(Ctx& cx, const float* frames, int F, int H, int W, const std::vector<int>& src, const std::vector<int>& tgt, int iters,
                             const float* flow_init, const RaftOutputs& o, bool gather) {
-  if (!serves_raft()) throw std::runtime_error("gimmvfi: no RAFT weights were loaded (finalize_weights_raft / finalize_weights)");
   if (F < 1) throw std::runtime_error("raft: at least one frame is required");
   if (H % 8 || W % 8 || H < 128 || W < 128)   // (the 4-level pyramid halves H/8 three times: raft/corr.py:23-44 divides by zero below 128)
     throw std::runtime_error("raft: frames must be a multiple of 8 and >= 128 in each dimension (got " + std::to_string(H) + "x" + std::to_string(W) + ")");
@@ -1728,6 +1722,7 @@ void Engine::run_raft_pairs(Ctx& cx, const float* frames, int F, int H, int W, c
 }
 
 size_t Engine::plan_raft(int n_frames, int h, int w, int n_pairs, int outputs) {
+  need(Entry::Raft);
   if (n_pairs < 1) throw std::runtime_error("raft: at least one pair is required");
   if (n_frames < 1) throw std::runtime_error("raft: at least one frame is required");
   if (outputs & ~GIMMVFI_RAFT_OUT_ITERS) throw std::runtime_error("raft: unknown output flags");
@@ -1736,18 +1731,14 @@ size_t Engine::plan_raft(int n_frames, int h, int w, int n_pairs, int outputs) {
   // flow_init, and the gathering path only adds buffers: a change that breaks either must change this plan too.
   std::vector<int> src(n_pairs), tgt(n_pairs);
   for (int s = 0; s < n_pairs; ++s) { src[s] = s % n_frames; tgt[s] = (s + 1) % n_frames; }
-  Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  float* fake = reinterpret_cast<float*>(size_t(64));
-  RaftOutputs o; o.flow_up = o.flow_low = o.feat4 = o.feat8 = o.fmap = fake;
-  if (outputs & GIMMVFI_RAFT_OUT_ITERS) o.flow_iters = fake;
-  const bool dbg = debug_; debug_ = false;
-  run_raft_pairs(cx, fake, n_frames, h, w, src, tgt, 1, nullptr, o, true);
-  debug_ = dbg; taps_.clear();
-  return cx.arena.peak + 256;
+  RaftOutputs o; o.flow_up = o.flow_low = o.feat4 = o.feat8 = o.fmap = kFake;
+  if (outputs & GIMMVFI_RAFT_OUT_ITERS) o.flow_iters = kFake;
+  return dry_run([&](Ctx& cx) { run_raft_pairs(cx, kFake, n_frames, h, w, src, tgt, 1, nullptr, o, true); });
 }
 
 void Engine::forward_raft(const float* frames, int n_frames, int h, int w, const int32_t* pairs, int n_pairs, int iters, const float* flow_init,
                           const RaftOutputs& out, void* workspace, size_t workspace_bytes, gvStream_t stream) {
+  need(Entry::Raft);
   if (!frames || !pairs) throw std::runtime_error("raft: frames and pairs are required");
   if (n_pairs < 1) throw std::runtime_error("raft: at least one pair is required");
   if (iters < 1) throw std::runtime_error("raft: iters must be >= 1");
@@ -1758,16 +1749,7 @@ void Engine::forward_raft(const float* frames, int n_frames, int h, int w, const
       throw std::runtime_error("raft: pair " + std::to_string(s) + " = (" + std::to_string(src[s]) + ", " + std::to_string(tgt[s]) +
                                ") indexes outside the " + std::to_string(n_frames) + " frames");
   }
-  DeviceGuard dg(device_);
-  Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
-  prof_.reset();
-  cx.prof = profile_ ? &prof_ : nullptr;
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255);
-  cx.arena.base = reinterpret_cast<char*>(base);
-  cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
-  taps_.clear();
-  run_raft_pairs(cx, frames, n_frames, h, w, src, tgt, iters, flow_init, out, false);
-  launches_ = cx.launches;
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run_raft_pairs(cx, frames, n_frames, h, w, src, tgt, iters, flow_init, out, false); });
 }
 
 // ---------------------------------------------------------------------------
@@ -1779,10 +1761,7 @@ static const int kLpipsShape[5][4] = {{64, 3, 11, 11}, {192, 64, 5, 5}, {384, 19
 
 void Engine::finalize_weights_lpips() {
   DeviceGuard dg(device_);
-  for (void* p : dev_allocs_) dev_free(p);
-  dev_allocs_.clear(); conv_.clear(); vec_.clear();
-  fc_valid_.clear(); ++weights_version_; clear_graphs();
-  finalized_ = false;
+  drop_weights();
   auto expect = [&](const std::string& key, std::vector<int64_t> shape) {
     const HostTensor& t = raw(key);
     if (t.shape != shape) throw std::runtime_error("gimmvfi: LPIPS weight '" + key + "' has an unexpected shape");
@@ -1814,7 +1793,7 @@ void Engine::finalize_weights_lpips() {
   for (int k = 1; k < 5; ++k) pack_conv(kLpipsConv[k]);
   vec("scaling_layer.shift"); vec("scaling_layer.scale");
   for (int k = 0; k < 5; ++k) vec("lin" + std::to_string(k) + ".model.1.weight");
-  finalized_ = true; gimm_only_ = false; synth_only_ = false; ff_ = false; lpips_ = true; ff_only_ = false; raft_only_ = false;
+  held_ = Weights::Lpips;
 }
 
 void Engine::run_lpips(Ctx& cx, int n, int h, int w, const LpipsIO& io) {
@@ -1858,29 +1837,16 @@ void Engine::run_lpips(Ctx& cx, int n, int h, int w, const LpipsIO& io) {
 }
 
 size_t Engine::plan_lpips(int n, int h, int w) {
-  if (!finalized_ || !lpips_) throw std::runtime_error("gimmvfi: no LPIPS weights were loaded (finalize_weights_lpips)");
-  Ctx cx; cx.dry = true; cx.arena.dry = true; cx.sm_count = sm_count_;
-  LpipsIO io; float* fake = reinterpret_cast<float*>(size_t(64));
-  io.in0 = io.in1 = io.out = fake;
-  const bool dbg = debug_; debug_ = false;
-  run_lpips(cx, n, h, w, io);
-  debug_ = dbg; taps_.clear();
-  return cx.arena.peak + 256;
+  need(Entry::Lpips);
+  LpipsIO io;
+  io.in0 = io.in1 = io.out = kFake;
+  return dry_run([&](Ctx& cx) { run_lpips(cx, n, h, w, io); });
 }
 
 void Engine::forward_lpips(int n, int h, int w, const LpipsIO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
-  if (!finalized_ || !lpips_) throw std::runtime_error("gimmvfi: no LPIPS weights were loaded (finalize_weights_lpips)");
+  need(Entry::Lpips);
   if (!io.in0 || !io.in1 || !io.out) throw std::runtime_error("lpips: in0, in1 and out are required");
-  DeviceGuard dg(device_);
-  Ctx cx; cx.stream = stream; cx.sm_count = sm_count_;
-  prof_.reset();
-  cx.prof = profile_ ? &prof_ : nullptr;
-  uintptr_t base = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255);
-  cx.arena.base = reinterpret_cast<char*>(base);
-  cx.arena.cap = workspace_bytes - (base - reinterpret_cast<uintptr_t>(workspace));
-  taps_.clear();
-  run_lpips(cx, n, h, w, io);
-  launches_ = cx.launches;
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run_lpips(cx, n, h, w, io); });
 }
 
 }  // namespace gv

@@ -102,6 +102,10 @@ struct Net;
 
 class Engine {
  public:
+  // the weight set the last finalize_weights* loaded (None: none yet, weights loaded since, or a finalize that failed part-way)
+  enum class Weights { None, R, F, Synthesis, Gimm, Raft, FlowFormer, Lpips };
+  // the entry points, grouped by the weight sets that serve them (the table in need())
+  enum class Entry { Interpolate, FromFlow, Gimm, Raft, FlowFormer, Lpips };
   explicit Engine(int device);
   ~Engine();
   void load_weight(const std::string& key, const float* host, const int64_t* shape, int ndim);
@@ -159,7 +163,7 @@ class Engine {
   std::string last_error;
   int raft_iters = 20;  // GIMMVFI_R hard-codes iters=20 (gimmvfi_r.py:126-132)
   int ff_iters = 32;    // FlowFormer decoder_depth (flowformer/configs/submission.py:50; gimmvfi_f.py:115 passes iters=None)
-  bool is_f() const { return ff_; }
+  bool is_f() const { return held_ == Weights::F; }
   const float* ff_c1w() const { return ff_c1w_.data(); }   // first cost-map patch-embedding layer, [36 taps][16] and [16] (host copies)
   const float* ff_c1b() const { return ff_c1b_.data(); }
   // debug taps from the estimator's helpers (flowformer.cu)
@@ -169,10 +173,14 @@ class Engine {
   int device() const { return device_; }
   int64_t weights_version() const { return weights_version_; }
   const void* hyponet_blob(bool fp32_class) const { return fp32_class ? hypo_blob3_ : hypo_blob_; }   // bumped by every finalize_weights*: callers key caches on it
-  bool finalized() const { return finalized_; }
+  void need(Entry e) const;   // throws unless the weights held serve e
 
  private:
   struct Impl;
+  void drop_weights();
+  void prefix_flow_estimator(std::initializer_list<const char*> children);
+  size_t dry_run(const std::function<void(Ctx&)>& run);
+  void launch(void* workspace, size_t workspace_bytes, gvStream_t stream, const std::function<void(Ctx&)>& run);
   void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr);
   void finalize_decoders();
   void finalize_flowformer();
@@ -186,16 +194,9 @@ class Engine {
   void run_raft(Ctx& cx, Net& N, const RaftRun& r);
   void run_raft_pairs(Ctx& cx, const float* frames, int n_frames, int h, int w, const std::vector<int>& src, const std::vector<int>& tgt, int iters,
                       const float* flow_init, const RaftOutputs& o, bool gather);
-  bool serves_raft() const { return finalized_ && (raft_only_ || (!gimm_only_ && !synth_only_ && !ff_ && !lpips_ && !ff_only_)); }
-  void refuse_raft_only() const { if (raft_only_) throw std::runtime_error("gimmvfi: this engine holds RAFT weights only (finalize_weights_raft); use forward_raft"); }
-  bool raft_only_ = false;
-  void refuse_ff_only() const { if (ff_only_) throw std::runtime_error("gimmvfi: this engine holds FlowFormer weights only (finalize_weights_flowformer); use forward_flowformer"); }
-  bool ff_only_ = false;
   void run_gimm(Ctx& cx, const Problem& p, const GimmIO& io);
   void finalize_gimm_part();
   void run_lpips(Ctx& cx, int n, int h, int w, const LpipsIO& io);
-  void refuse_lpips() const { if (lpips_) throw std::runtime_error("gimmvfi: this engine holds LPIPS weights (finalize_weights_lpips); use forward_lpips"); }
-  bool lpips_ = false;
   void gimm_encode(Net& N, const TV& nf, const TV& f01, const TV& f10, const TV& wts, const TV& X64);
   void gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, const TV& wts, const float* tdev, const float* coords_t, const TV& ninr,
                    bool tap_it);
@@ -206,7 +207,8 @@ class Engine {
   void tap(const std::string& name, const TV& tv) { if (debug_) taps_[name] = tv; }
 
   int device_ = 0;
-  bool finalized_ = false, debug_ = false, profile_ = false, gimm_only_ = false, synth_only_ = false, ff_ = false;
+  Weights held_ = Weights::None;
+  bool debug_ = false, profile_ = false;
   int tc_mode_ = 0;
   int64_t weights_version_ = 0;
   bool use_graph_ = false;

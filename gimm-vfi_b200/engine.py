@@ -67,7 +67,6 @@ class EngineHandle:
             self.device = torch.device("cuda", idx)
         self._ws = None
         self._plans: Dict[tuple, int] = {}
-        self.weights_loaded = False
         # static_outputs: forward() returns the same output tensors on every call of a problem shape (overwritten by the next call) -
         # with set_cuda_graph(True) and caller-owned input tensors this makes every pointer repeat, i.e. every forward a graph replay
         self.static_outputs = False
@@ -82,6 +81,10 @@ class EngineHandle:
             pass
 
     # ------------------------------------------------------------------ weights
+    _FINALIZE = {"gimm_only": "gimmvfi_finalize_weights_gimm", "synthesis_only": "gimmvfi_finalize_weights_synthesis",
+                 "full_f": "gimmvfi_finalize_weights_f", "lpips": "gimmvfi_finalize_weights_lpips",
+                 "flowformer": "gimmvfi_finalize_weights_flowformer", "raft": "gimmvfi_finalize_weights_raft"}
+
     def load_state_dict(self, sd: Dict[str, torch.Tensor], gimm_only: bool = False, synthesis_only: bool = False, full_f: bool = False,
                         lpips: bool = False, flowformer: bool = False, raft: bool = False):
         """gimm_only: `sd` is a standalone GIMM checkpoint (gimm.py's module tree), only gimm_forward() is available.
@@ -92,7 +95,13 @@ class EngineHandle:
         flowformer: `sd` is the FlowFormer module's state_dict (GIMM-VFI-F's flow_estimator.*, prefix stripped or not); only
         flowformer_forward() is available (a full_f engine serves it too).
         raft: `sd` is the RAFT module's state_dict (GIMM-VFI-R's flow_estimator.*, prefix stripped); only raft_forward() is available
-        (a full GIMM-VFI-R engine serves it too)."""
+        (a full GIMM-VFI-R engine serves it too).
+        None of them: `sd` is a complete GIMM-VFI-R state_dict.  At most one may be set."""
+        chosen = [k for k, on in dict(gimm_only=gimm_only, synthesis_only=synthesis_only, full_f=full_f, lpips=lpips, flowformer=flowformer,
+                                      raft=raft).items() if on]
+        if len(chosen) > 1:
+            raise ValueError("load_state_dict: %s select different weight sets; set at most one" % " and ".join(chosen))
+        fin = getattr(self.lib.dll, self._FINALIZE[chosen[0]] if chosen else "gimmvfi_finalize_weights")
         for k, v in sd.items():
             if not v.dtype.is_floating_point:
                 continue  # num_batches_tracked
@@ -101,12 +110,7 @@ class EngineHandle:
             t = v.detach().to("cpu", torch.float32).contiguous()
             shape = (C.c_int64 * max(t.dim(), 1))(*t.shape)
             self.lib.check(self.lib.dll.gimmvfi_load_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()), self._h)
-        fin = self.lib.dll.gimmvfi_finalize_weights_raft if raft else self.lib.dll.gimmvfi_finalize_weights_flowformer if flowformer else self.lib.dll.gimmvfi_finalize_weights_lpips if lpips else self.lib.dll.gimmvfi_finalize_weights_gimm if gimm_only else (
-            self.lib.dll.gimmvfi_finalize_weights_synthesis if synthesis_only else (
-                self.lib.dll.gimmvfi_finalize_weights_f if full_f else self.lib.dll.gimmvfi_finalize_weights))
-        self.synthesis_only = synthesis_only
         self.lib.check(fin(self._h), self._h)
-        self.weights_loaded = True
 
     def set_debug(self, on: bool):
         self.lib.check(self.lib.dll.gimmvfi_set_debug(self._h, int(on)), self._h)
@@ -136,8 +140,7 @@ class EngineHandle:
         """Per-kernel CUDA-event totals of the last forward (set_profile(True) first)."""
         import json
 
-        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
-        return json.loads(self.lib.dll.gimmvfi_profile_json(self._h, C.c_void_p(stream)).decode())
+        return json.loads(self.lib.dll.gimmvfi_profile_json(self._h, self._stream()).decode())
 
     def set_raft_iters(self, iters: int):
         self.lib.check(self.lib.dll.gimmvfi_set_raft_iters(self._h, int(iters)), self._h)
@@ -166,20 +169,32 @@ class EngineHandle:
         """torch's current device = the engine's for the duration of a call (stream lookup, torch.empty)"""
         return torch.cuda.device(self._index) if self.device.type == "cuda" else contextlib.nullcontext()
 
+    def _stream(self) -> C.c_void_p:
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None)
+
+    def _plan(self, key, plan_call) -> int:
+        """workspace bytes of the call that key identifies: plan_call(size_t*) calls the plan export, once per key"""
+        if key not in self._plans:
+            n = C.c_size_t()
+            self.lib.check(plan_call(C.byref(n)), self._h)
+            self._plans[key] = int(n.value)
+        return self._plans[key]
+
+    def _workspace(self, nbytes: int) -> torch.Tensor:
+        """the engine's workspace, grown to at least nbytes"""
+        if self._ws is None or self._ws.numel() < nbytes:
+            self._ws = None
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self._ws
+
     # ------------------------------------------------------------------ forward
     def _problem(self, B, Hf, Wf, T, ds, Hc, Wc) -> Problem:
         return Problem(B, Hf, Wf, T, float(ds) if ds else 0.0, Hc, Wc)
 
     def workspace_bytes(self, B, Hf, Wf, T, ds, Hc, Wc, from_flow: bool = False) -> int:
         key = (B, Hf, Wf, T, float(ds) if ds else 0.0, Hc, Wc)
-        pkey = key + (bool(from_flow),)
-        if pkey not in self._plans:
-            p = self._problem(*key)
-            n = C.c_size_t()
-            plan = self.lib.dll.gimmvfi_plan_from_flow if from_flow else self.lib.dll.gimmvfi_plan
-            self.lib.check(plan(self._h, C.byref(p), C.byref(n)), self._h)
-            self._plans[pkey] = int(n.value)
-        return self._plans[pkey]
+        plan = self.lib.dll.gimmvfi_plan_from_flow if from_flow else self.lib.dll.gimmvfi_plan
+        return self._plan(key + (bool(from_flow),), lambda n: plan(self._h, C.byref(self._problem(*key)), n))
 
     def frame_cache_bytes(self, B, Hf, Wf, T, ds, Hc, Wc) -> int:
         p = self._problem(B, Hf, Wf, T, ds, Hc, Wc)
@@ -205,10 +220,7 @@ class EngineHandle:
         B, _, _, Hf, Wf = img_xs.shape
         T, _, _, Hc, Wc, _ = coords.shape
         H, W = (Hf, Wf) if not ds else (int(Hf * ds), int(Wf * ds))
-        nbytes = self.workspace_bytes(B, Hf, Wf, T, ds, Hc, Wc, from_flow=flow_inputs is not None)
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self._workspace(self.workspace_bytes(B, Hf, Wf, T, ds, Hc, Wc, from_flow=flow_inputs is not None))
         E = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
         if aux_outputs is None or isinstance(aux_outputs, (bool, int)):
             aux = _ENGINE_AUX if aux_outputs else ()
@@ -242,7 +254,6 @@ class EngineHandle:
         for k, v in out.items():
             setattr(io, k, v.data_ptr())
         p = self._problem(B, Hf, Wf, T, ds, Hc, Wc)
-        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
         if frame_cache is not None:
             buf, load, store = frame_cache
             assert buf.dtype == torch.uint8 and buf.is_contiguous() and buf.device == self.device
@@ -254,10 +265,10 @@ class EngineHandle:
                 for j in range(2):
                     f.feat4[j], f.feat8[j], f.fnet[j] = (flow_inputs[k][j].data_ptr() for k in ("feat4", "feat8", "fnet"))
                 self.lib.check(self.lib.dll.gimmvfi_forward_from_flow(self._h, C.byref(p), C.byref(io), C.byref(f), C.c_void_p(self._ws.data_ptr()),
-                                                                      self._ws.numel(), C.c_void_p(stream)), self._h)
+                                                                      self._ws.numel(), self._stream()), self._h)
             else:
                 self.lib.check(self.lib.dll.gimmvfi_forward(self._h, C.byref(p), C.byref(io), C.c_void_p(self._ws.data_ptr()),
-                                                            self._ws.numel(), C.c_void_p(stream)), self._h)
+                                                            self._ws.numel(), self._stream()), self._h)
         finally:
             if frame_cache is not None:
                 self.lib.check(self.lib.dll.gimmvfi_set_frame_cache(self._h, None, 0, 0, 0), self._h)
@@ -278,20 +289,11 @@ class EngineHandle:
         Hc, Wc = coords.shape[3], coords.shape[4]
         assert tuple(ori_flow.shape) == (B, 2, 2, H, W) and tuple(t.shape) == (T, B)
         p = self._problem(B, H, W, T, None, Hc, Wc)
-        key = ("gimm", B, H, W, T, Hc, Wc)
-        if key not in self._plans:
-            n = C.c_size_t()
-            self.lib.check(self.lib.dll.gimmvfi_gimm_plan(self._h, C.byref(p), C.byref(n)), self._h)
-            self._plans[key] = int(n.value)
-        nbytes = self._plans[key]
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self._workspace(self._plan(("gimm", B, H, W, T, Hc, Wc), lambda n: self.lib.dll.gimmvfi_gimm_plan(self._h, C.byref(p), n)))
         out = torch.empty(T, B, 2, 1, Hc, Wc, dtype=torch.float32, device=self.device)
-        stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
         P = lambda x: C.c_void_p(x.data_ptr())
-        self.lib.check(self.lib.dll.gimmvfi_gimm_forward(self._h, C.byref(p), P(xs), P(ori_flow), P(coords), P(t), P(out), P(self._ws),
-                                                         self._ws.numel(), C.c_void_p(stream)), self._h)
+        self.lib.check(self.lib.dll.gimmvfi_gimm_forward(self._h, C.byref(p), P(xs), P(ori_flow), P(coords), P(t), P(out), P(ws),
+                                                         ws.numel(), self._stream()), self._h)
         return out
 
     def lpips_forward(self, in0: torch.Tensor, in1: torch.Tensor, normalize: bool = False, quantize: bool = False, per_layer: bool = False):
@@ -302,22 +304,13 @@ class EngineHandle:
             raise ValueError("lpips: in0 and in1 must both be (n,3,h,w), got %s and %s" % (tuple(in0.shape), tuple(in1.shape)))
         n, _, h, w = in0.shape
         with self._guard():
-            key = ("lpips", n, h, w)
-            if key not in self._plans:
-                nb = C.c_size_t()
-                self.lib.check(self.lib.dll.gimmvfi_lpips_plan(self._h, n, h, w, C.byref(nb)), self._h)
-                self._plans[key] = int(nb.value)
-            nbytes = self._plans[key]
-            if self._ws is None or self._ws.numel() < nbytes:
-                self._ws = None
-                self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            ws = self._workspace(self._plan(("lpips", n, h, w), lambda nb: self.lib.dll.gimmvfi_lpips_plan(self._h, n, h, w, nb)))
             out = torch.empty(n, dtype=torch.float32, device=self.device)
             layers = torch.empty(n, 5, dtype=torch.float32, device=self.device) if per_layer else None
-            stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
             P = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
             flags = (1 if normalize else 0) | (2 if quantize else 0)
-            self.lib.check(self.lib.dll.gimmvfi_lpips_forward(self._h, P(in0), P(in1), n, h, w, flags, P(out), P(layers), P(self._ws),
-                                                              self._ws.numel(), C.c_void_p(stream)), self._h)
+            self.lib.check(self.lib.dll.gimmvfi_lpips_forward(self._h, P(in0), P(in1), n, h, w, flags, P(out), P(layers), P(ws),
+                                                              ws.numel(), self._stream()), self._h)
         return (out, layers) if per_layer else out
 
     def flowformer_forward(self, frames: torch.Tensor, pairs, pairs_per_call: int = 1, iters: int = 0, flow_low: bool = False):
@@ -334,21 +327,12 @@ class EngineHandle:
         P = len(pl)
         flat = (C.c_int32 * max(2 * P, 1))(*[i for ab in pl for i in ab])
         with self._guard():
-            key = ("flowformer", F, H, W, P)
-            if key not in self._plans:
-                nb = C.c_size_t()
-                self.lib.check(self.lib.dll.gimmvfi_flowformer_plan(self._h, F, H, W, P, C.byref(nb)), self._h)
-                self._plans[key] = int(nb.value)
-            nbytes = self._plans[key]
-            if self._ws is None or self._ws.numel() < nbytes:
-                self._ws = None
-                self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            ws = self._workspace(self._plan(("flowformer", F, H, W, P), lambda nb: self.lib.dll.gimmvfi_flowformer_plan(self._h, F, H, W, P, nb)))
             up = torch.empty(P, 2, H, W, dtype=torch.float32, device=self.device)
             low = torch.empty(P, 2, H // 8, W // 8, dtype=torch.float32, device=self.device) if flow_low else None
-            stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
             Pt = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
             self.lib.check(self.lib.dll.gimmvfi_flowformer_forward(self._h, Pt(frames), F, H, W, flat, P, int(pairs_per_call), int(iters), Pt(up),
-                                                                   Pt(low), Pt(self._ws), self._ws.numel(), C.c_void_p(stream)), self._h)
+                                                                   Pt(low), Pt(ws), ws.numel(), self._stream()), self._h)
         return (up, low) if flow_low else up
 
     RAFT_OUTPUTS = ("flow_up", "flow_low", "flow_iters", "feat4", "feat8", "fmap")
@@ -375,23 +359,15 @@ class EngineHandle:
         flat = (C.c_int32 * max(2 * P, 1))(*[i for ab in pl for i in ab])
         with self._guard():
             want_iters = "flow_iters" in outputs
-            key = ("raft", F, H, W, P, want_iters)
-            if key not in self._plans:
-                nb = C.c_size_t()
-                self.lib.check(self.lib.dll.gimmvfi_raft_plan(self._h, F, H, W, P, int(want_iters), C.byref(nb)), self._h)
-                self._plans[key] = int(nb.value)
-            nbytes = self._plans[key]
-            if self._ws is None or self._ws.numel() < nbytes:
-                self._ws = None
-                self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            plan = lambda nb: self.lib.dll.gimmvfi_raft_plan(self._h, F, H, W, P, int(want_iters), nb)
+            ws = self._workspace(self._plan(("raft", F, H, W, P, want_iters), plan))
             shapes = dict(flow_up=(P, 2, H, W), flow_low=(P, 2, H // 8, W // 8), flow_iters=(max(iters, 0), P, 2, H, W),
                           feat4=(P, 96, H // 4, W // 4), feat8=(P, 128, H // 8, W // 8), fmap=(P, 256, H // 8, W // 8))
             out = {k: torch.empty(*shapes[k], dtype=torch.float32, device=self.device) for k in self.RAFT_OUTPUTS if k in outputs}
-            stream = torch.cuda.current_stream(self.device).cuda_stream if self.device.type == "cuda" else None
             Pt = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
             self.lib.check(self.lib.dll.gimmvfi_raft_forward(self._h, Pt(frames), F, H, W, flat, P, iters, Pt(flow_init),
-                                                             *[Pt(out.get(k)) for k in self.RAFT_OUTPUTS], Pt(self._ws), self._ws.numel(),
-                                                             C.c_void_p(stream)), self._h)
+                                                             *[Pt(out.get(k)) for k in self.RAFT_OUTPUTS], Pt(ws), ws.numel(), self._stream()),
+                           self._h)
         return out
 
     def tap(self, name: str) -> torch.Tensor:
