@@ -158,6 +158,13 @@ def param_spec_r() -> Spec:
 
 
 R_ONLY_PREFIXES = ("flow_estimator.", "amt_last_cproj.", "amt_second_last_cproj.", "amt_fproj.")
+ESTIMATOR_PREFIX = "flow_estimator."
+
+
+def strip_prefix(spec: Spec) -> Spec:
+    """the `flow_estimator.*` entries of a GIMM-VFI spec in registration order, prefix stripped: the spec of the estimator module
+    alone (RAFT for param_spec_r, FlowFormer for param_spec_f)"""
+    return [(k[len(ESTIMATOR_PREFIX):], s, dt) for k, s, dt in spec if k.startswith(ESTIMATOR_PREFIX)]
 
 
 def param_spec_f() -> Spec:

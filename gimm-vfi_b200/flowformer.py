@@ -10,77 +10,26 @@ Memory per pair: the cost volume and the GMA attention matrix are N^2 floats eac
 from typing import Optional, Sequence, Tuple
 
 import torch
-import torch.nn as nn
 
-from .arch import param_spec_f
-from .engine import EngineHandle
-from .model import _Node
+from .arch import ESTIMATOR_PREFIX, param_spec_f, strip_prefix
+from .module import EngineModule, load_estimator_checkpoint
 from .weights import random_state_dict_f
 
-PREFIX = "flow_estimator."
+load_flowformer_checkpoint = load_estimator_checkpoint
 
 
 def param_spec_flowformer():
     """(key, shape, dtype) of the reference FlowFormer module: GIMM-VFI-F's flow_estimator.* in registration order, prefix stripped"""
-    return [(k[len(PREFIX):], s, dt) for k, s, dt in param_spec_f() if k.startswith(PREFIX)]
+    return strip_prefix(param_spec_f())
 
 
-def load_flowformer_checkpoint(path_or_dict) -> dict:
-    """initialize_Flowformer's convert (flowformer/__init__.py): keep the keys containing "module" and drop "module." from them.
-    Takes a path (torch.load on the CPU, e.g. flowformer_sintel.pth, the checkpoint GIMM-VFI-F loads, configs/submission.py:17) or
-    an already loaded dict."""
-    ckpt = torch.load(path_or_dict, map_location="cpu") if isinstance(path_or_dict, str) else path_or_dict
-    return {k.replace("module.", ""): v for k, v in ckpt.items() if "module" in k}
-
-
-class FlowFormer(nn.Module):
+class FlowFormer(EngineModule):
     def __init__(self, cfg=None, seed: int = 0):
-        super().__init__()
+        super().__init__(flowformer=True)
         self.cfg = cfg
-        init = random_state_dict_f(seed)
-        for key, shape, dt in param_spec_flowformer():
-            parts = key.split(".")
-            mod = self
-            for p in parts[:-1]:
-                if p not in mod._modules:
-                    mod.add_module(p, _Node())
-                mod = mod._modules[p]
-            t = init[PREFIX + key].clone()
-            if dt == "int64":
-                mod.register_buffer(parts[-1], t)
-            else:
-                mod.register_parameter(parts[-1], nn.Parameter(t, requires_grad=False))
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
+        self.build_params(param_spec_flowformer(), random_state_dict_f(seed), ESTIMATOR_PREFIX)
         # 4 (default): the 3xF16 fp32-class tensor-core forms, ~2e-3 px from the reference; 0: fp32 CUDA cores, ~2e-4 px
         self.tensor_cores = 4
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
-
-    @property
-    def engine(self) -> EngineHandle:
-        dev = self.memory_decoder.proj.weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("FlowFormer (gimmvfi_b200) runs on CUDA devices only; call model.to('cuda') first — there is no CPU path")
-        if self._engine is None or self._engine.device != dev or self._weights_dirty:
-            if self._engine is None or self._engine.device != dev:
-                self._engine = EngineHandle(dev)
-            self._engine.load_state_dict(self.state_dict(), flowformer=True)
-            self._engine.tensor_cores = None
-            self._weights_dirty = False
-        return self._engine
-
-    def _ready(self, x: torch.Tensor) -> EngineHandle:
-        if x.device.type != "cuda":
-            raise RuntimeError("FlowFormer (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
-        eng = self.engine
-        if getattr(eng, "tensor_cores", None) != int(self.tensor_cores):
-            eng.set_tensor_cores(int(self.tensor_cores))
-        return eng
 
     @torch.no_grad()
     def forward(self, image1, image2, output=None, flow_init=None, return_feat=False, iters=None) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -2,15 +2,11 @@
 alone: bidirectional flows in, the normalised flow at time t out (SURVEY.md 8(f) row 4).  Same constructor argument, same
 ``forward(xs, coord, keep_xs_shape, ori_flow, timesteps)`` signature, same 36-key ``state_dict``; ``forward`` is one call
 into the sm_90a engine (the kernels of the GIMM stages of GIMM-VFI-R, csrc/engine.cu gimm_encode / gimm_decode).  CUDA only."""
-from typing import Optional
-
 import torch
-import torch.nn as nn
 
 from .arch import param_spec_r
-from .config import default_arch_config
 from .engine import EngineHandle
-from .model import _Node, sample_coords
+from .model import _GIMMBase
 from .weights import random_state_dict
 
 GIMM_KEY_PREFIXES = ("g_filter", "alpha_v", "alpha_fe", "cnn_encoder.", "res_conv.", "hyponet.")
@@ -25,52 +21,11 @@ def param_spec_gimm():
     return sorted(spec, key=lambda e: rank(e[0]))   # stable: keeps the order inside each group
 
 
-class GIMM(nn.Module):
+class GIMM(_GIMMBase):
     def __init__(self, config=None, seed: int = 0):
-        super().__init__()
-        self.config = config = (config.copy() if config is not None else default_arch_config())
-        self.hyponet_config = config.hyponet
-        self.fwarp_type = getattr(config, "fwarp_type", "linear")
-        if self.fwarp_type != "linear":
-            raise NotImplementedError("only fwarp_type='linear' (configs.py:44) is built")
-        self.coord_range = list(config.coord_range)
-        init = random_state_dict(seed)
-        for key, shape, dt in param_spec_gimm():
-            parts = key.split(".")
-            mod = self
-            for p in parts[:-1]:
-                if p not in mod._modules:
-                    mod.add_module(p, _Node())
-                mod = mod._modules[p]
-            mod.register_parameter(parts[-1], nn.Parameter(init[key].clone(), requires_grad=False))
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
+        super().__init__(config, gimm_only=True)
+        self.build_params(param_spec_gimm(), random_state_dict(seed))
         self.tensor_cores = 1   # 0: fp32 CUDA cores; >= 1: TF32 wgmma (everything here is downstream of RAFT, DESIGN.md precision plan)
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
-
-    @property
-    def engine(self) -> EngineHandle:
-        if self._engine is None or self._weights_dirty:
-            dev = self.g_filter.device
-            if dev.type != "cuda":
-                raise RuntimeError("GIMM (gimmvfi_b200) runs on CUDA devices only; call model.to('cuda') first — there is no CPU path")
-            if self._engine is None or self._engine.device != dev:
-                self._engine = EngineHandle(dev)
-            self._engine.load_state_dict(self.state_dict(), gimm_only=True)
-            self._engine.tensor_cores = None
-            self._weights_dirty = False
-        return self._engine
-
-    def sample_coord_input(self, batch_size, s_shape, t_ids, coord_range=None, upsample_ratio=1.0, device=None):
-        """gimm.py:239-253"""
-        assert device is not None
-        assert coord_range is None
-        return sample_coords(batch_size, s_shape, t_ids, self.coord_range, upsample_ratio, device)
 
     @torch.no_grad()
     def forward(self, xs, coord=None, keep_xs_shape=True, ori_flow=None, timesteps=None):
@@ -80,17 +35,12 @@ class GIMM(nn.Module):
         In the list form the grids may differ in size: one engine call per distinct size (see gimm_forward_grids)."""
         if coord is None or ori_flow is None or timesteps is None:
             raise ValueError("GIMM.forward needs coord, ori_flow and timesteps (the reference's coord=None default cannot run either, gimm.py:132)")
-        if xs.device.type != "cuda":
-            raise RuntimeError("GIMM (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
+        eng = self._ready(xs)
         is_list = isinstance(timesteps, list)
         if is_list:
             assert isinstance(coord, list)
             assert len(timesteps) == len(coord)
         cl, tl = (coord, timesteps) if is_list else ([coord], [timesteps])
-        B = xs.shape[0]
-        eng = self.engine
-        if getattr(eng, "tensor_cores", None) != int(self.tensor_cores):
-            eng.set_tensor_cores(int(self.tensor_cores))
         out = gimm_forward_grids(eng, xs, ori_flow, cl, tl)   # [(B,2,1,Hc,Wc)]
         outs = [o if keep_xs_shape else o.permute(0, 2, 3, 4, 1) for o in out]
         return outs if is_list else outs[0]

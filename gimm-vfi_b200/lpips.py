@@ -8,7 +8,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .engine import EngineHandle
+from .module import EngineModule
 
 CHANNELS = (64, 192, 384, 256, 256)
 # torchvision AlexNet `features` index -> the LPIPS module's key (pretrained_networks.py:70-110 slices features[0:12] into 5 slices)
@@ -58,7 +58,7 @@ class _AlexFeatures(nn.Module):
             p.requires_grad = False
 
 
-class LPIPS(nn.Module):
+class LPIPS(EngineModule):
     """``LPIPS(net="alex", version="0.1")`` with the reference's state_dict (22 keys, see lpips_keys()) and forward.
 
     Only the configuration calc_lpips builds exists: net="alex", version="0.1", lpips=True, spatial=False; anything else raises
@@ -66,7 +66,7 @@ class LPIPS(nn.Module):
     or lpips_state_dict() / load_lpips() from torchvision's AlexNet file and the reference's alex.pth).  CUDA tensors only."""
 
     def __init__(self, net: str = "alex", version: str = "0.1", lpips: bool = True, spatial: bool = False):
-        super().__init__()
+        super().__init__(lpips=True)
         if net != "alex":
             raise NotImplementedError("LPIPS (gimmvfi_b200): only net='alex' is built (got %r)" % (net,))
         if version != "0.1":
@@ -83,26 +83,7 @@ class LPIPS(nn.Module):
         for p in self.parameters():
             p.requires_grad = False
         self.eval()
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
-
-    @property
-    def engine(self) -> EngineHandle:
-        if self._engine is None or self._weights_dirty:
-            dev = self.scaling_layer.shift.device
-            if dev.type != "cuda":
-                raise RuntimeError("LPIPS (gimmvfi_b200) runs on CUDA devices only; call .to('cuda') first — there is no CPU path")
-            if self._engine is None or self._engine.device != dev:
-                self._engine = EngineHandle(dev)
-            self._engine.load_state_dict(self.state_dict(), lpips=True)
-            self._weights_dirty = False
-        return self._engine
+        self._track_loads()
 
     def _prepare(self, x: torch.Tensor, name: str) -> torch.Tensor:
         if not torch.is_tensor(x) or not x.is_cuda:

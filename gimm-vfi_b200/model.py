@@ -4,45 +4,33 @@ gimmvfi_r.py:34-507).  Same constructor argument (``config.arch`` node), same
 414-key ``state_dict`` — but ``forward`` is one call into the sm_90a engine through
 the C ABI.  CUDA only; there is no PyTorch / CPU fallback path.
 """
-import weakref
-from typing import List, Optional
-
 import torch
 import torch.nn as nn
 
 from .arch import param_spec_r
 from .config import default_arch_config
-from .engine import AUX_OUTPUTS, EngineHandle, aux_keys, model_outputs
+from .engine import AUX_OUTPUTS, aux_keys, model_outputs
+from .module import EngineModule, _RootRef
 from .weights import random_state_dict
-
-
-class _Node(nn.Module):
-    """Anonymous container used to reproduce the reference's module tree names."""
 
 
 class _FlowEstimator(nn.Module):
     """GIMMVFI_R.flow_estimator: the RAFT module's parameter tree (gimmvfi_r.py:45), callable with RAFT.forward (raft/raft.py:100-169)
-    through the model's own engine, so the weights are not loaded twice.  The model is held by a weak reference, not registered as a
+    through the model's own engine, so the weights are not loaded twice.  The model is held by a _RootRef, not registered as a
     submodule: the state_dict, its order and its sharing are the reference's."""
 
     hidden_dim = context_dim = 128
 
     def __init__(self, model):
         super().__init__()
-        self.__dict__["_model"] = weakref.ref(model)
+        self.__dict__["_model"] = _RootRef(model)
 
     @torch.no_grad()
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False, return_feat=True):
         """RAFT.forward's three return forms, as gimmvfi_b200.RAFT.forward; `upsample` is ignored, as in the reference."""
         from .raft import raft_forward
 
-        model = self.__dict__["_model"]()
-        if image1.device.type != "cuda":
-            raise RuntimeError("GIMMVFI_R.flow_estimator (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
-        eng = model.engine
-        if getattr(eng, "tensor_cores", None) != int(model.tensor_cores):
-            eng.set_tensor_cores(int(model.tensor_cores))
-        return raft_forward(eng, image1, image2, iters, flow_init, test_mode, return_feat)
+        return raft_forward(self.__dict__["_model"]()._ready(image1), image1, image2, iters, flow_init, test_mode, return_feat)
 
 
 def sample_coords(batch_size, s_shape, t_ids, coord_range=(-1.0, 1.0), upsample_ratio=1.0, device=None):
@@ -57,36 +45,35 @@ def sample_coords(batch_size, s_shape, t_ids, coord_range=(-1.0, 1.0), upsample_
     return g.unsqueeze(0).repeat(batch_size, 1, 1, 1, 1)
 
 
-class GIMMVFI_R(nn.Module):
-    def __init__(self, config=None, seed: int = 0):
-        super().__init__()
+class _GIMMBase(EngineModule):
+    """GIMM, GIMMVFI_R and GIMMVFI_F: the `config.arch` node they are built from and the reference's sample_coord_input."""
+
+    def __init__(self, config, **weight_set):
+        super().__init__(**weight_set)
         self.config = config = (config.copy() if config is not None else default_arch_config())
         self.hyponet_config = config.hyponet
-        self.raft_iter = 20  # gimmvfi_r.py:41 (config.raft_iter is ignored by the reference too)
-        self.num_flows = 3
         self.fwarp_type = getattr(config, "fwarp_type", "linear")
         if self.fwarp_type != "linear":
             raise NotImplementedError("only fwarp_type='linear' (the shipped configs' default, configs.py:44) is built")
         self.coord_range = list(config.coord_range)
-        init = random_state_dict(seed)
-        shared = {}
-        for key, shape, dt in param_spec_r():
-            mod, leaf = self._container(key)
-            alias = key.replace(".downsample.1.", ".norm3.") if ".downsample.1." in key else None
-            if alias is not None and alias in shared:  # norm3 and downsample.1 are one module (raft/extractor.py:44-47)
-                obj = shared[alias]
-            elif dt == "int64" or leaf in ("running_mean", "running_var"):
-                obj = init[key].clone()
-            else:
-                obj = nn.Parameter(init[key].clone(), requires_grad=False)
-            shared[key] = obj
-            if isinstance(obj, nn.Parameter):
-                mod.register_parameter(leaf, obj)
-            else:
-                mod.register_buffer(leaf, obj)
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
+
+    def sample_coord_input(self, batch_size, s_shape, t_ids, coord_range=None, upsample_ratio=1.0, device=None):
+        """gimm.py:239-253, gimmvfi_r.py:428-442, gimmvfi_f.py:391-407"""
+        assert device is not None
+        assert coord_range is None
+        return sample_coords(batch_size, s_shape, t_ids, self.coord_range, upsample_ratio, device)
+
+
+class _VFIBase(_GIMMBase):
+    """GIMMVFI_R and GIMMVFI_F: a whole interpolation is one engine forward, returning the reference's dict."""
+
+    # whether the engine runs RAFT's encoders, whose products a frame cache keeps (GIMMVFI_R).  Without them the cache would do nothing
+    # but turn off the engine's CUDA-graph replay, so _interpolate does not hand it on.
+    _raft_encoders = False
+
+    def __init__(self, config, **weight_set):
+        super().__init__(config, **weight_set)
+        self.num_flows = 3
         # True: every auxiliary output; False: imgt_pred only; or a collection of keys of the returned dict, e.g. ("flowt",):
         # imgt_pred plus those (the engine allocates and writes only what is selected)
         self.aux_outputs = True
@@ -97,69 +84,60 @@ class GIMMVFI_R(nn.Module):
         # trunk and the decoder concat in fp16 storage.  All modes meet max|d imgt_pred| <= 1e-3 vs the reference.
         self.tensor_cores = 4
 
-    def _container(self, key: str):
-        parts = key.split(".")
-        mod = self
-        for p in parts[:-1]:
-            if p not in mod._modules:
-                mod.add_module(p, _FlowEstimator(self) if mod is self and p == "flow_estimator" else _Node())
-            mod = mod._modules[p]
-        return mod, parts[-1]
+    @staticmethod
+    def _check_args(coord, t):
+        """the inference form of the reference forward's coord and t (gimmvfi_r.py:324-367, gimmvfi_f.py:304-343)"""
+        assert isinstance(t, list)
+        assert isinstance(coord, list)
+        assert len(t) == len(coord)
+        for c in coord:
+            assert isinstance(c, tuple)
+            if c[1] is not None:
+                raise NotImplementedError("sub-sampled coordinates are the training path (gimmvfi_r.py:358-367, gimmvfi_f.py:334-343); "
+                                          "inference passes None")
 
-    # ---------------------------------------------------------------- engine plumbing
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
+    def _external_flows(self, xs, ds_factor):
+        """flow_inputs for the engine when the estimator runs outside it (GIMMVFI_F.flow_backend); None: the engine's own"""
+        return None
 
-    def refresh_weights(self):
-        """Re-pack + upload the weights (automatic after load_state_dict / .to())."""
-        dev = self.g_filter.device
-        if dev.type != "cuda":
-            raise RuntimeError("GIMMVFI_R (gimmvfi_b200) runs on CUDA devices only; call model.to('cuda') first — there is no CPU path")
-        if self._engine is None or self._engine.device != dev:
-            self._engine = EngineHandle(dev)
-        self._engine.load_state_dict(self.state_dict())
-        self._weights_dirty = False
-        self._engine.tensor_cores = None
+    def _interpolate(self, img_xs, coord, t, ds_factor, aux, frame_cache=None, flow_inputs=None):
+        """forward's body.  aux: an aux_outputs selection; frame_cache: see EngineHandle.forward, used by GIMMVFI_R only (the RAFT
+        encoders' products); flow_inputs: precomputed estimator outputs, as GIMMVFI_F.cal_bidirection_flow returns them."""
+        eng = self._ready(img_xs)
+        B = img_xs.shape[0]
+        xs = img_xs.to(torch.float32).contiguous()
+        if flow_inputs is None:
+            flow_inputs = self._external_flows(xs, ds_factor)
+        coords = torch.stack([c[0].to(torch.float32) for c in coord], 0).contiguous()  # (T,B,1,Hc,Wc,3)
+        tt = torch.stack([x.reshape(-1).to(torch.float32).expand(B) for x in t], 0).contiguous()  # (T,B)
+        keys = aux_keys(aux)
+        o = eng.forward(xs, coords, tt, ds_factor, aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]],
+                        frame_cache=frame_cache if self._raft_encoders else None, flow_inputs=flow_inputs)
+        return model_outputs(o, len(t), keys)
 
-    @property
-    def engine(self) -> EngineHandle:
-        if self._engine is None or self._weights_dirty:
-            self.refresh_weights()
-        return self._engine
+    def compute_psnr(self, preds, targets, reduction="mean"):
+        """gimmvfi_r.py:412-426 (the same in gimmvfi_f.py)"""
+        assert reduction in ["mean", "sum", "none"]
+        mse = torch.reshape((preds - targets) ** 2, (preds.shape[0], -1)).mean(dim=-1)
+        psnr = -10 * torch.log10(mse)
+        return psnr.mean() if reduction == "mean" else (psnr.sum() if reduction == "sum" else psnr)
 
-    # ---------------------------------------------------------------- reference API
-    def sample_coord_input(self, batch_size, s_shape, t_ids, coord_range=None, upsample_ratio=1.0, device=None):
-        """gimmvfi_r.py:428-442"""
-        assert device is not None
-        assert coord_range is None
-        return sample_coords(batch_size, s_shape, t_ids, self.coord_range, upsample_ratio, device)
+
+class GIMMVFI_R(_VFIBase):
+    _raft_encoders = True
+
+    def __init__(self, config=None, seed: int = 0):
+        super().__init__(config)
+        self.raft_iter = 20  # gimmvfi_r.py:41 (config.raft_iter is ignored by the reference too)
+        self.flow_estimator = _FlowEstimator(self)   # the first child in the reference's order; build_params fills it
+        self.build_params(param_spec_r(), random_state_dict(seed))
 
     @torch.no_grad()
     def forward(self, img_xs, coord=None, t=None, iters=None, ds_factor=None):
         """gimmvfi_r.py:324-407 (inference form).  ``iters`` is accepted and ignored, as in
         the reference (cal_bidirection_flow hard-codes 20, gimmvfi_r.py:126-132)."""
-        assert isinstance(t, list)
-        assert isinstance(coord, list)
-        assert len(t) == len(coord)
-        assert coord is not None
-        for c in coord:
-            assert isinstance(c, tuple)
-            if c[1] is not None:
-                raise NotImplementedError("sub-sampled coordinates are the training path (gimmvfi_r.py:358-367); inference passes None")
-        if img_xs.device.type != "cuda":
-            raise RuntimeError("GIMMVFI_R (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
-        eng = self.engine
-        if getattr(eng, "tensor_cores", None) != int(self.tensor_cores):
-            eng.set_tensor_cores(int(self.tensor_cores))
-        B = img_xs.shape[0]
-        xs = img_xs.to(torch.float32).contiguous()
-        coords = torch.stack([c[0].to(torch.float32) for c in coord], 0).contiguous()  # (T,B,1,Hc,Wc,3)
-        tt = torch.stack([x.reshape(-1).to(torch.float32).expand(B) for x in t], 0).contiguous()  # (T,B)
-        keys = aux_keys(self.aux_outputs)
-        o = eng.forward(xs, coords, tt, ds_factor, aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]], frame_cache=getattr(self, "_frame_cache", None))
-        return model_outputs(o, len(t), keys)
+        self._check_args(coord, t)
+        return self._interpolate(img_xs, coord, t, ds_factor, self.aux_outputs)
 
     def warp_frame(self, frame, flow):
         """gimmvfi_r.py:409-410 — backward warp of an NCHW frame by an NCHW flow."""
@@ -174,13 +152,6 @@ class GIMMVFI_R(nn.Module):
         s = C.c_void_p(torch.cuda.current_stream(src.device).cuda_stream)
         lib.check(lib.dll.gimmvfi_op_backwarp(C.byref(view_of(src)), C.byref(view_of(fl)), C.byref(view_of(dst)), s))
         return dst.permute(0, 3, 1, 2).contiguous()
-
-    def compute_psnr(self, preds, targets, reduction="mean"):
-        """gimmvfi_r.py:412-426"""
-        assert reduction in ["mean", "sum", "none"]
-        mse = torch.reshape((preds - targets) ** 2, (preds.shape[0], -1)).mean(dim=-1)
-        psnr = -10 * torch.log10(mse)
-        return psnr.mean() if reduction == "mean" else (psnr.sum() if reduction == "sum" else psnr)
 
 
 def _check_engine_config(config):

@@ -13,73 +13,22 @@ Everything runs natively on the sm_90a engine (``gimmvfi_finalize_weights_f`` + 
 from typing import Callable, Optional
 
 import torch
-import torch.nn as nn
 
-from .arch import param_spec_f
-from .config import default_arch_config
-from .engine import AUX_OUTPUTS, EngineHandle, aux_keys, model_outputs
-from .model import _Node, sample_coords
+from .arch import ESTIMATOR_PREFIX, param_spec_f
+from .model import _VFIBase
 from .weights import random_state_dict_f
 
 
-class GIMMVFI_F(nn.Module):
+class GIMMVFI_F(_VFIBase):
     def __init__(self, config=None, seed: int = 0):
-        super().__init__()
-        self.config = config = (config.copy() if config is not None else default_arch_config())
-        self.hyponet_config = config.hyponet
-        self.raft_iter = getattr(config, "raft_iter", 20)
-        self.num_flows = 3
-        self.fwarp_type = getattr(config, "fwarp_type", "linear")
-        if self.fwarp_type != "linear":
-            raise NotImplementedError("only fwarp_type='linear' (the shipped configs' default, configs.py:44) is built")
-        self.coord_range = list(config.coord_range)
-        init = random_state_dict_f(seed)
-        for key, shape, dt in param_spec_f():
-            parts = key.split(".")
-            mod = self
-            for p in parts[:-1]:
-                if p not in mod._modules:
-                    mod.add_module(p, _Node())
-                mod = mod._modules[p]
-            leaf = parts[-1]
-            if dt == "int64" or leaf in ("running_mean", "running_var"):
-                mod.register_buffer(leaf, init[key].clone())
-            else:
-                mod.register_parameter(leaf, nn.Parameter(init[key].clone(), requires_grad=False))
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
-        self.aux_outputs = True   # as GIMMVFI_R.aux_outputs
-        self.tensor_cores = 4
+        super().__init__(config, full_f=True)
+        self.raft_iter = getattr(self.config, "raft_iter", 20)
+        self.build_params(param_spec_f(), random_state_dict_f(seed))
         self.flow_backend: Optional[Callable] = None   # see the module docstring
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
-
-    @property
-    def engine(self) -> EngineHandle:
-        dev = self.g_filter.device
-        if dev.type != "cuda":
-            raise RuntimeError("GIMMVFI_F (gimmvfi_b200) runs on CUDA devices only; there is no CPU path")
-        if self._engine is None or self._engine.device != dev or self._weights_dirty:
-            if self._engine is None or self._engine.device != dev:
-                self._engine = EngineHandle(dev)
-            self._engine.load_state_dict(self.state_dict(), full_f=True)
-            self._engine.tensor_cores = None
-            self._weights_dirty = False
-        return self._engine
 
     def flow_estimator_state_dict(self) -> dict:
         """`flow_estimator.*` with the prefix stripped: what the reference FlowFormer module's load_state_dict takes."""
-        return {k[len("flow_estimator."):]: v for k, v in self.state_dict().items() if k.startswith("flow_estimator.")}
-
-    def sample_coord_input(self, batch_size, s_shape, t_ids, coord_range=None, upsample_ratio=1.0, device=None):
-        """gimmvfi_f.py:391-407"""
-        assert device is not None
-        assert coord_range is None
-        return sample_coords(batch_size, s_shape, t_ids, self.coord_range, upsample_ratio, device)
+        return {k[len(ESTIMATOR_PREFIX):]: v for k, v in self.state_dict().items() if k.startswith(ESTIMATOR_PREFIX)}
 
     def cal_bidirection_flow(self, im0, im1):
         """gimmvfi_f.py:114-138 through an EXTERNAL flow backend (model.flow_backend) -> the dict gimmvfi_forward_from_flow takes.
@@ -91,38 +40,17 @@ class GIMMVFI_F(nn.Module):
         f10 = f10[0] if isinstance(f10, (list, tuple)) else f10
         return dict(flows=torch.stack([f01, f10], 2), feat4=[feats0[0], feats1[0]], feat8=[feats0[1], feats1[1]], fnet=[fnet0, fnet1])
 
+    def _external_flows(self, xs, ds_factor):
+        if self.flow_backend is None:
+            return None
+        x_net = xs
+        if ds_factor is not None:   # gimmvfi_f.py:309-318: the estimator sees the down-scaled frames
+            rs = lambda a: torch.nn.functional.interpolate(a, scale_factor=ds_factor, mode="bilinear", align_corners=False)
+            x_net = torch.stack([rs(xs[:, :, 0]), rs(xs[:, :, 1])], 2)
+        return self.cal_bidirection_flow(255 * x_net[:, :, 0], 255 * x_net[:, :, 1])
+
     @torch.no_grad()
     def forward(self, img_xs, coord=None, t=None, ds_factor=None, flow_inputs=None):
         """gimmvfi_f.py:304-384 (inference form).  `flow_inputs` (optional) = precomputed outputs of cal_bidirection_flow."""
-        assert isinstance(t, list)
-        assert isinstance(coord, list)
-        assert len(t) == len(coord)
-        for c in coord:
-            assert isinstance(c, tuple)
-            if c[1] is not None:
-                raise NotImplementedError("sub-sampled coordinates are the training path (gimmvfi_f.py:334-343); inference passes None")
-        if img_xs.device.type != "cuda":
-            raise RuntimeError("GIMMVFI_F (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
-        eng = self.engine
-        if getattr(eng, "tensor_cores", None) != int(self.tensor_cores):
-            eng.set_tensor_cores(int(self.tensor_cores))
-        B = img_xs.shape[0]
-        xs = img_xs.to(torch.float32).contiguous()
-        if flow_inputs is None and self.flow_backend is not None:
-            x_net = xs
-            if ds_factor is not None:   # gimmvfi_f.py:309-318: the estimator sees the down-scaled frames
-                rs = lambda a: torch.nn.functional.interpolate(a, scale_factor=ds_factor, mode="bilinear", align_corners=False)
-                x_net = torch.stack([rs(xs[:, :, 0]), rs(xs[:, :, 1])], 2)
-            flow_inputs = self.cal_bidirection_flow(255 * x_net[:, :, 0], 255 * x_net[:, :, 1])
-        coords = torch.stack([c[0].to(torch.float32) for c in coord], 0).contiguous()
-        tt = torch.stack([x.reshape(-1).to(torch.float32).expand(B) for x in t], 0).contiguous()
-        keys = aux_keys(self.aux_outputs)
-        o = eng.forward(xs, coords, tt, ds_factor, aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]], flow_inputs=flow_inputs)
-        return model_outputs(o, len(t), keys)
-
-    def compute_psnr(self, preds, targets, reduction="mean"):
-        """gimmvfi_f.py:389-..."""
-        assert reduction in ["mean", "sum", "none"]
-        mse = torch.reshape((preds - targets) ** 2, (preds.shape[0], -1)).mean(dim=-1)
-        psnr = -10 * torch.log10(mse)
-        return psnr.mean() if reduction == "mean" else (psnr.sum() if reduction == "sum" else psnr)
+        self._check_args(coord, t)
+        return self._interpolate(img_xs, coord, t, ds_factor, self.aux_outputs, flow_inputs=flow_inputs)

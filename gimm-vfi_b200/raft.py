@@ -9,29 +9,21 @@ and change nothing (the correlation is the volume pyramid, or the volume-free lo
 device).  CUDA only.
 
 Memory per pair: the volume pyramid is N^2 * 4/3 floats, N = (H/8)(W/8): 0.5 GB at 544x960, 8.5 GB at 1088x1920."""
-from typing import Optional, Sequence, Tuple
+from typing import Sequence, Tuple
 
 import torch
-import torch.nn as nn
 
-from .arch import param_spec_r
+from .arch import ESTIMATOR_PREFIX, param_spec_r, strip_prefix
 from .engine import EngineHandle
-from .model import _Node
+from .module import EngineModule, load_estimator_checkpoint
 from .weights import random_state_dict
 
-PREFIX = "flow_estimator."
+load_raft_checkpoint = load_estimator_checkpoint
 
 
 def param_spec_raft():
     """(key, shape, dtype) of the reference RAFT module: GIMM-VFI-R's flow_estimator.* in registration order, prefix stripped"""
-    return [(k[len(PREFIX):], s, dt) for k, s, dt in param_spec_r() if k.startswith(PREFIX)]
-
-
-def load_raft_checkpoint(path_or_dict) -> dict:
-    """initialize_RAFT's convert (raft/__init__.py:16-19): keep the keys containing "module" and drop "module." from them.  Takes a path
-    (torch.load on the CPU, e.g. raft-things.pth, the checkpoint GIMM-VFI-R's estimator starts from) or an already loaded dict."""
-    ckpt = torch.load(path_or_dict, map_location="cpu") if isinstance(path_or_dict, str) else path_or_dict
-    return {k.replace("module.", ""): v for k, v in ckpt.items() if "module" in k}
+    return strip_prefix(param_spec_r())
 
 
 def raft_forward(eng: EngineHandle, image1, image2, iters=12, flow_init=None, test_mode=False, return_feat=True):
@@ -53,66 +45,17 @@ def raft_forward(eng: EngineHandle, image1, image2, iters=12, flow_init=None, te
     return list(o["flow_iters"].unbind(0))
 
 
-class RAFT(nn.Module):
+class RAFT(EngineModule):
     def __init__(self, args=None, seed: int = 0):
-        super().__init__()
+        super().__init__(raft=True)
         if args is not None and getattr(args, "small", False):
             raise NotImplementedError("RAFT (gimmvfi_b200): args.small=True is RAFT-small, a different network; the engine builds the full "
                                       "RAFT of GIMM-VFI-R (raft.py:38-44, 64-70)")
         self.args = args
         self.hidden_dim = self.context_dim = 128
-        init = random_state_dict(seed)
-        shared = {}
-        for key, shape, dt in param_spec_raft():
-            parts = key.split(".")
-            mod = self
-            for p in parts[:-1]:
-                if p not in mod._modules:
-                    mod.add_module(p, _Node())
-                mod = mod._modules[p]
-            alias = key.replace(".downsample.1.", ".norm3.") if ".downsample.1." in key else None
-            if alias is not None and alias in shared:   # norm3 and downsample.1 are one module (raft/extractor.py:44-47)
-                obj = shared[alias]
-            elif dt == "int64" or parts[-1] in ("running_mean", "running_var"):
-                obj = init[PREFIX + key].clone()
-            else:
-                obj = nn.Parameter(init[PREFIX + key].clone(), requires_grad=False)
-            shared[key] = obj
-            if isinstance(obj, nn.Parameter):
-                mod.register_parameter(parts[-1], obj)
-            else:
-                mod.register_buffer(parts[-1], obj)
-        self._engine: Optional[EngineHandle] = None
-        self._weights_dirty = True
-        self.register_load_state_dict_post_hook(lambda m, k: setattr(m, "_weights_dirty", True))
+        self.build_params(param_spec_raft(), random_state_dict(seed), ESTIMATOR_PREFIX)
         # 4 (default, as GIMM-VFI-R): RAFT on the fp32-class 3xF16 / 3xTF32 tensor-core forms; 0: fp32 CUDA cores
         self.tensor_cores = 4
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._weights_dirty = True
-        return r
-
-    @property
-    def engine(self) -> EngineHandle:
-        dev = self.fnet.conv1.weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("RAFT (gimmvfi_b200) runs on CUDA devices only; call model.to('cuda') first — there is no CPU path")
-        if self._engine is None or self._engine.device != dev or self._weights_dirty:
-            if self._engine is None or self._engine.device != dev:
-                self._engine = EngineHandle(dev)
-            self._engine.load_state_dict(self.state_dict(), raft=True)
-            self._engine.tensor_cores = None
-            self._weights_dirty = False
-        return self._engine
-
-    def _ready(self, x: torch.Tensor) -> EngineHandle:
-        if x.device.type != "cuda":
-            raise RuntimeError("RAFT (gimmvfi_b200): inputs must live on a CUDA device; there is no CPU path")
-        eng = self.engine
-        if getattr(eng, "tensor_cores", None) != int(self.tensor_cores):
-            eng.set_tensor_cores(int(self.tensor_cores))
-        return eng
 
     @torch.no_grad()
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False, return_feat=True):

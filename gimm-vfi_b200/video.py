@@ -82,12 +82,7 @@ def interpolate_pair_u8(model, frame0_u8: torch.Tensor, frame1_u8: torch.Tensor,
     ratio = 1.0 if ds_factor is None else ds_factor
     coords = [(model.sample_coord_input(1, (H, W), [i / N], device=dev, upsample_ratio=ratio), None) for i in range(1, N)]
     ts = [i / N * torch.ones(1, device=dev) for i in range(1, N)]
-    aux = model.aux_outputs
-    model.aux_outputs = ("flowt",) if with_flow else False
-    try:
-        out = model(xs, coords, t=ts, ds_factor=ds_factor)
-    finally:
-        model.aux_outputs = aux
+    out = model._interpolate(xs, coords, ts, ds_factor, ("flowt",) if with_flow else False)
     frames = [padder.unpad_u8(im, bgr)[0] for im in out["imgt_pred"]]
     return (frames, flow_images(padder, out["flowt"], bgr)) if with_flow else frames
 
@@ -131,26 +126,22 @@ class VideoInterpolator:
         need = m.engine.frame_cache_bytes(1, H, W, N - 1, self.ds, Hc, Wc)
         if self._cache is None or self._cache.numel() < need or self._cache.device != dev:
             self._cache, self._cache_valid = torch.empty(need, dtype=torch.uint8, device=dev), False
-        aux, m.aux_outputs = m.aux_outputs, (("flowt",) if self.with_flow else False)
+        aux = ("flowt",) if self.with_flow else False
         # The engine keeps its own record of what each cache buffer holds (problem size, precision mode; cleared when the weights
         # change): a refused load -> one full forward with load=False.  The signature adds what only the caller can know.
         sig = (id(m.engine), int(m.tensor_cores), m.engine.weights_version)
         load = self._cache_valid and getattr(self, "_cache_sig", None) == sig
         try:
             try:
-                m._frame_cache = (self._cache, load, True)
-                out = m(xs, coords, t=ts, ds_factor=self.ds)
+                out = m._interpolate(xs, coords, ts, self.ds, aux, frame_cache=(self._cache, load, True))
             except GimmvfiError as ex:
                 if not (load and "frame cache" in str(ex)):
                     raise
-                m._frame_cache = (self._cache, False, True)
-                out = m(xs, coords, t=ts, ds_factor=self.ds)
+                out = m._interpolate(xs, coords, ts, self.ds, aux, frame_cache=(self._cache, False, True))
             self._cache_valid, self._cache_sig = True, sig
         except Exception:
             self._cache_valid = False
             raise
-        finally:
-            m.aux_outputs, m._frame_cache = aux, None
         self._prev = cur
         frames = [self._padder.unpad_u8(im, self.bgr)[0] for im in out["imgt_pred"]]
         return (frames, flow_images(self._padder, out["flowt"], self.bgr)) if self.with_flow else frames

@@ -88,11 +88,8 @@ def test_frame_cache_is_bit_exact_on_gpu(weights0):
     t = [0.5 * torch.ones(1, device=DEV)]
     ref_bc = m(pair(Bf, Cf), coord, t=t)
     cache = torch.zeros(m.engine.frame_cache_bytes(1, H, W, 1, None, H, W), dtype=torch.uint8, device=DEV)
-    m._frame_cache = (cache, False, True)
-    m(pair(A, Bf), coord, t=t)
-    m._frame_cache = (cache, True, True)
-    got_bc = m(pair(Bf, Cf), coord, t=t)
-    m._frame_cache = None
+    m._interpolate(pair(A, Bf), coord, t, None, m.aux_outputs, frame_cache=(cache, False, True))
+    got_bc = m._interpolate(pair(Bf, Cf), coord, t, None, m.aux_outputs, frame_cache=(cache, True, True))
     assert torch.equal(ref_bc["raft_flow"], got_bc["raft_flow"])
     assert (ref_bc["imgt_pred"][0] - got_bc["imgt_pred"][0]).abs().max().item() <= 6e-4
 
