@@ -1210,7 +1210,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     N.conv(p + "7", d, fup1, ACT_RELU);
     A.release(mk);
   }
-  tap("syn.feat4", feat4);
+  tap("syn.feat4", feat4); tap("syn.feat8", feat8); tap("syn.fup4", fup4); tap("syn.fproj", fproj);
   tap_copy(cx, "syn.fup1", fup1);   // (half in mode 4)
 
   // ------------------------------------------------------------ GIMM (t-independent part)  gimmvfi_r.py:158-168
@@ -1236,10 +1236,12 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   const size_t t_mark = A.mark();
   for (int ti = 0; ti < T; ++ti) {
     A.release(t_mark);
+    // debug taps of the per-timestep tensors are taken at the last timestep: nothing overwrites them after it
+    const bool last = ti == T - 1;
     const float* tdev = io.t + (int64_t)ti * B;
     TV ninr = A.tensor(B, H, W, 2);
     cx.tc_split = (knobs & 1) != 0;
-    gimm_decode(N, X64, f01, f10, wts, tdev, io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3, ninr, ti == 0);
+    gimm_decode(N, X64, f01, f10, wts, tdev, io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3, ninr, last);
     cx.tc_split = (knobs & 4) != 0;   // init decoder + update blocks
     if (io.ninrflow) nhwc_to_nchw(cx, ninr, io.ninrflow + (int64_t)ti * B * 2 * H * W, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
     TV flow_t = A.tensor(B, H, W, 2);
@@ -1269,6 +1271,10 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     TV ft_4 = o136.slice(0, 128);
     TV fl4 = A.tensor(B, H4, W4, 4), mask4 = A.tensor(B, H4, W4, 1);
     flow_mask_split(cx, o136, f0in, f1in, fl4.slice(0, 2), fl4.slice(2, 2), mask4);
+    if (last) {   // (ft_4 / fl4 are updated in place by the update blocks: snapshots)
+      tap("syn.fin4", fin); tap("syn.mask4_init", mask4);
+      tap_copy(cx, "syn.ft4_init", ft_4); tap_copy(cx, "syn.fl4_init", fl4);
+    }
     // warp_w_mask(scale=4) -> img_warp_4 (aux output, gimmvfi_r.py:259-261)
     if (io.img_warp_4) {
       const size_t mk = A.mark();
@@ -1296,13 +1302,14 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       }
     }
     amt_update(N, "amt_update4_low", true, ft_4, fl4, grid_flow, corr648);
+    if (last) { tap("syn.corr648", corr648); tap_copy(cx, "syn.ft4_low", ft_4); tap_copy(cx, "syn.fl4_low", fl4); }
     {
       TV corr_hi = A.tensor(B, H4, W4, 648);
       resize_bilinear(cx, corr648, corr_hi, 0.5f, 0.5f, 1.f, 0, ACT_NONE);  // gimmvfi_r.py:274
       amt_update(N, "amt_update4_high", false, ft_4, fl4, fl4, corr_hi);
-      if (ti == 0) tap("syn.corr_4_hi", corr_hi);
+      if (last) tap("syn.corr_4_hi", corr_hi);
     }
-    if (ti == 0) { tap("syn.ft_4", ft_4); tap("syn.fl4", fl4); tap("syn.mask4", mask4); }
+    if (last) { tap("syn.ft_4", ft_4); tap("syn.fl4", fl4); tap("syn.mask4", mask4); }
     if (io.flowt0_4) nhwc_to_nchw(cx, fl4.slice(0, 2), io.flowt0_4 + (int64_t)ti * B * 2 * H4 * W4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
     if (io.flowt1_4) nhwc_to_nchw(cx, fl4.slice(2, 2), io.flowt1_4 + (int64_t)ti * B * 2 * H4 * W4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
 
@@ -1310,7 +1317,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     cx.tc_split = (knobs & 8) != 0;
     TV F0 = A.tensor(B, H, W, 6, 8), F1 = A.tensor(B, H, W, 6, 8), Mk = A.tensor(B, H, W, 3, 4), Rs = A.tensor(B, H, W, 9, 12);
     // debug snapshots of the concat, the fp32 flows / mask and convblock.4's output: allocated here, outside the block that frees them
-    const bool snap = debug_ && ti == 0;
+    const bool snap = debug_ && last;
     TV fin1_snap = snap ? A.tensor(B, H, W, 273) : TV(), aux5_snap = snap && half_chains(cx) ? A.tensor(B, H, W, 5) : TV();
     TV o24_snap = snap ? A.tensor(B, H, W, 24) : TV();
     {
@@ -1347,7 +1354,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       final_heads(cx, o24, fl0, fl1, mk1, F0, F1, Mk, Rs);
       A.release(mk);
     }
-    if (ti == 0) { tap("syn.F0", F0); tap("syn.F1", F1); tap("syn.Mk", Mk); tap("syn.Rs", Rs); }
+    if (last) { tap("syn.F0", F0); tap("syn.F1", F1); tap("syn.Mk", Mk); tap("syn.Rs", Rs); }
     cx.tc_split = (knobs & 16) != 0;   // comb block
     TV F0f = F0, F1f = F1, Mkf = Mk, Rsf = Rs;
     if (ds) {  // gimmvfi_r.py:294-303
@@ -1359,7 +1366,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       resize_bilinear(cx, wide(F1), wide(F1f), rinv, rinv, inv, 0, ACT_NONE);
       resize_bilinear(cx, wide(Mk), wide(Mkf), rinv, rinv, 1.f, 0, ACT_NONE);
       resize_bilinear(cx, wide(Rs), wide(Rsf), rinv, rinv, 1.f, 0, ACT_NONE);
-      if (ti == 0) { tap("syn.F0f", F0f); tap("syn.F1f", F1f); tap("syn.Mkf", Mkf); tap("syn.Rsf", Rsf); }
+      if (last) { tap("syn.F0f", F0f); tap("syn.F1f", F1f); tap("syn.Mkf", Mkf); tap("syn.Rsf", Rsf); }
     }
     if (io.flowt0_1) nhwc_to_nchw(cx, F0f, io.flowt0_1 + (int64_t)ti * B * 6 * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
     if (io.flowt1_1) nhwc_to_nchw(cx, F1f, io.flowt1_1 + (int64_t)ti * B * 6 * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
@@ -1370,7 +1377,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       N.conv7x("amt_comb_block.0", w9, c18, ACT_PRELU, N.V("amt_comb_block.1.weight"));
       N.conv7x("amt_comb_block.2", c18, c3);
       combine_output(cx, mean3, c3, io.imgt_pred + (int64_t)ti * B * 3 * Hf * Wf);
-      if (ti == 0) { tap("syn.w9", w9); tap("syn.mean3", mean3); tap("syn.c3", c3); }
+      if (last) { tap("syn.w9", w9); tap("syn.mean3", mean3); tap("syn.c3", c3); }
     }
     cx.tc_split = false;
   }
@@ -1405,7 +1412,7 @@ void Engine::gimm_encode(Net& N, const TV& nf /*2B: [nf01; nf10]*/, const TV& f0
     N.conv("cnn_encoder.7", x.batch(B, B), X64.slice(16, 16), ACT_NONE, nullptr, 1, true);
     A.release(mk);
   }
-  tap("gimm.lat0", X64.slice(0, 16));
+  tap("gimm.lat0", X64.slice(0, 16)); tap("gimm.lat1", X64.slice(16, 16));
 }
 
 // one timestep: forward splat of both latents to time t, latent refiner, HypoNet -> normalised flow ninr (B,Hc,Wc,2) on the coordinate grid
@@ -1427,7 +1434,7 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
     softsplat_normalize(cx, acc.batch(0, B), X64.slice(32, 16));
     softsplat_normalize(cx, acc.batch(B, B), X64.slice(48, 16));
   }
-  if (tap_it) tap("gimm.splat0", X64.slice(32, 16));
+  if (tap_it) { tap("gimm.splat0", X64.slice(32, 16)); tap("gimm.splat1", X64.slice(48, 16)); }
   // HypoNet (hyponet.py:71-146).  Tensor-core modes: ONE fused kernel (hyponet.cu) that takes the refined latent and the caller's
   // coordinate tensor directly; fp32 mode: five 1x1 convolutions on a packed [latent32 | t,y,x] input.
   // The coordinate grid (Hc, Wc) = ninr's size may differ from the flow resolution (GIMM standalone): HypoNet first resizes the
@@ -1515,7 +1522,7 @@ void Engine::run_gimm(Ctx& cx, const Problem& P, const GimmIO& io) {
   gimm_encode(N, nf, f01, f10, wts, X64);
   TV ninr = A.tensor(B, Hc, Wc, 2);
   for (int ti = 0; ti < T; ++ti) {
-    gimm_decode(N, X64, f01, f10, wts, io.t + (int64_t)ti * B, io.coords + (int64_t)ti * B * Hc * Wc * 3, ninr, ti == 0);
+    gimm_decode(N, X64, f01, f10, wts, io.t + (int64_t)ti * B, io.coords + (int64_t)ti * B * Hc * Wc * 3, ninr, ti == T - 1);
     nhwc_to_nchw(cx, ninr, io.out + (int64_t)ti * B * 2 * Hc * Wc, (int64_t)2 * Hc * Wc, (int64_t)Hc * Wc, 1.f, 0.f, 0);
   }
 }

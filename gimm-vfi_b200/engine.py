@@ -373,8 +373,10 @@ class EngineHandle:
     def tap(self, name: str) -> torch.Tensor:
         """Debug: copy of an intermediate NHWC tensor of the last forward (set_debug(True) first).
         Taps are read as float32: every tapped tensor is fp32 in all precision modes (the half-precision tensors of modes 3-4 that
-        are tapped - syn.fup1, syn.fin1 - are fp32 snapshots of the stored half values).  The per-timestep taps (gimm.splat0, gimm.latent, syn.*) are taken at the first timestep, and the buffers they
-        point into are reused by the following ones: read them after a forward with T = 1."""
+        are tapped - syn.fup1, syn.fin1 - are fp32 snapshots of the stored half values).  The per-timestep taps (gimm.splat0 / splat1,
+        gimm.latent, syn.* apart from syn.feat4 / feat8 / fup4 / fup1 / fproj) are taken at the LAST timestep, whose buffers nothing
+        overwrites after it.  Every timestep depends only on the t-independent state and its own t / coordinates, so to inspect a
+        timestep, put it last."""
         v = View()
         self.lib.check(self.lib.dll.gimmvfi_get_tap(self._h, name.encode(), C.byref(v)), self._h)
         base = self._ws.data_ptr()

@@ -136,7 +136,7 @@ def all_pairs_corr(f1: Tensor, f2: Tensor) -> Tensor:
     """raft/corr.py:167-175 / :85-93 → (B, h, w, 1, h, w)."""
     B, D, h, w = f1.shape
     c = torch.matmul(f1.view(B, D, h * w).transpose(1, 2), f2.view(B, D, h * w))
-    return c.view(B, h, w, 1, h, w) / torch.sqrt(torch.tensor(D).float())
+    return c.view(B, h, w, 1, h, w) / torch.sqrt(torch.tensor(D, device=c.device).to(c.dtype))
 
 
 def corr_pyramid(vol: Tensor, levels=4) -> List[Tensor]:
@@ -160,17 +160,18 @@ def _bilinear_sampler(img: Tensor, coords: Tensor) -> Tensor:
 
 def corr_lookup(pyr: List[Tensor], coords: Tensor, r=4) -> Tensor:
     """raft/corr.py:144-165.  ``delta = stack(meshgrid(dy, dx))`` is added to
-    (x, y): output channel i*9+j of a level samples offset (Δx, Δy)=(i-4, j-4)."""
+    (x, y): output channel i*9+j of a level samples offset (Δx, Δy)=(i-4, j-4).
+    On the coordinates' device, in the volume's dtype (float64 restatements)."""
     B, _, h1, w1 = coords.shape
     c = coords.permute(0, 2, 3, 1)
-    d = torch.linspace(-r, r, 2 * r + 1)
+    d = torch.linspace(-r, r, 2 * r + 1, device=coords.device, dtype=coords.dtype)
     delta = torch.stack(torch.meshgrid(d, d, indexing="ij"), dim=-1).view(1, 2 * r + 1, 2 * r + 1, 2)
     out = []
     for i, vol in enumerate(pyr):
         cen = c.reshape(B * h1 * w1, 1, 1, 2) / 2**i
         s = _bilinear_sampler(vol, cen + delta)
         out.append(s.view(B, h1, w1, -1))
-    return torch.cat(out, dim=-1).permute(0, 3, 1, 2).contiguous().float()
+    return torch.cat(out, dim=-1).permute(0, 3, 1, 2).contiguous().to(pyr[0].dtype)
 
 
 def raft_update_block(sd: SD, p: str, net: Tensor, inp: Tensor, corr: Tensor, flow: Tensor):
@@ -311,10 +312,11 @@ def res_conv(sd: SD, x: Tensor) -> Tensor:
 def forward_splat_sum(inp: Tensor, flow: Tensor) -> Tensor:
     """The ``softsplat_out`` CUDA kernel (modules/softsplat.py:376-421) restated
     with index_add_: every source pixel adds ``in·w_corner`` to its ≤4 in-frame
-    target corners; non-finite flow → pixel skipped."""
+    target corners; non-finite flow → pixel skipped.  On the input's device, in its dtype."""
     N, C, H, W = inp.shape
-    gx = torch.arange(W, dtype=inp.dtype).view(1, 1, W).expand(N, H, W)
-    gy = torch.arange(H, dtype=inp.dtype).view(1, H, 1).expand(N, H, W)
+    kw = dict(device=inp.device, dtype=inp.dtype)
+    gx = torch.arange(W, **kw).view(1, 1, W).expand(N, H, W)
+    gy = torch.arange(H, **kw).view(1, H, 1).expand(N, H, W)
     fx, fy = gx + flow[:, 0], gy + flow[:, 1]
     finite = torch.isfinite(fx) & torch.isfinite(fy)
     fx = torch.where(finite, fx, torch.zeros_like(fx))
@@ -328,8 +330,8 @@ def forward_splat_sum(inp: Tensor, flow: Tensor) -> Tensor:
         (x0, y1, (x1f - fx) * (fy - y0f)),
         (x1, y1, (fx - x0f) * (fy - y0f)),
     )
-    nidx = torch.arange(N).view(N, 1, 1).expand(N, H, W)
-    buf = torch.zeros(N * H * W, C, dtype=inp.dtype)
+    nidx = torch.arange(N, device=inp.device).view(N, 1, 1).expand(N, H, W)
+    buf = torch.zeros(N * H * W, C, **kw)
     src = inp.permute(0, 2, 3, 1).reshape(N * H * W, C)
     for xx, yy, ww in corners:
         ok = (finite & (xx >= 0) & (xx < W) & (yy >= 0) & (yy < H)).reshape(-1)
@@ -364,7 +366,7 @@ def hyponet_forward(sd: SD, coord: Tensor, latent_bhwc: Tensor, output_bias=0.5,
     hid = torch.cat([lat.reshape(B, -1, lat.shape[-1]), coord.view(B, -1, coord.shape[-1])], dim=-1)
     ws = hyponet_weights(sd)
     for i, (w, b) in enumerate(ws):
-        ones = torch.ones(*hid.shape[:-1], 1)
+        ones = torch.ones(*hid.shape[:-1], 1, device=hid.device, dtype=hid.dtype)
         hid = torch.bmm(torch.cat([hid, ones], -1), torch.cat([w, b], 0)[None].expand(B, -1, -1))
         if i < len(ws) - 1:
             hid = torch.sin(w0 * hid)
@@ -437,14 +439,22 @@ def _decoder_upsample(sd: SD, p: str, x: Tensor, n_shuffle: int) -> Tensor:
 
 def init_decoder(sd: SD, f0, f1, flow0_in, flow1_in, img0, img1):
     """fi_components.py:229-276"""
-    p = "amt_init_decoder"
-    f0 = _decoder_upsample(sd, p + ".upsample", f0, 1)
-    f1 = _decoder_upsample(sd, p + ".upsample", f1, 1)
-    f_in = torch.cat([backwarp(f0, flow0_in), backwarp(f1, flow1_in), flow0_in, flow1_in], 1)
+    f0 = _decoder_upsample(sd, "amt_init_decoder.upsample", f0, 1)
+    f1 = _decoder_upsample(sd, "amt_init_decoder.upsample", f1, 1)
+    return init_convblock(sd, init_decoder_concat(f0, f1, flow0_in, flow1_in, img0, img1), flow0_in, flow1_in)
+
+
+def init_decoder_concat(fup0, fup1, flow0_in, flow1_in, img0, img1):
+    """fi_components.py:255-268: the 272-channel convblock input from the up-sampled features and the flows at H/4"""
+    f_in = torch.cat([backwarp(fup0, flow0_in), backwarp(fup1, flow1_in), flow0_in, flow1_in], 1)
     sc = f_in.shape[2] / img0.shape[2]
     i0, i1 = resize(img0, sc), resize(img1, sc)
-    f_in = torch.cat([f_in, i0, i1, backwarp(i0, flow0_in), backwarp(i1, flow1_in)], 1)
-    c = p + ".convblock"
+    return torch.cat([f_in, i0, i1, backwarp(i0, flow0_in), backwarp(i1, flow1_in)], 1)
+
+
+def init_convblock(sd: SD, f_in, flow0_in, flow1_in):
+    """fi_components.py:269-276 -> (flow0, flow1, [mask | ft_])"""
+    c = "amt_init_decoder.convblock"
     x = _convrelu(sd, c + ".0", f_in, padding=0)
     for k in (1, 2, 3):
         x = _resblock(sd, "%s.%d" % (c, k), x, 64)

@@ -15,10 +15,10 @@ import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import gimmvfi_r_oracle as O
 from gimmvfi_b200.synth import synth_batch
+from splat_ref import splat_w_bound, splat_w_float64
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim"))
 
@@ -96,26 +96,6 @@ def check(engine_run, rows):
             bad.append(stage)
     print("\n%s mode %d\n  " % (kind, mode) + "\n  ".join(lines))
     assert not bad, "stages over their bar: %s\n%s" % (bad, "\n".join(lines))
-
-
-def splat_w_float64(sd, flows):
-    sd64 = {k: sd[k].double() for k in ("g_filter", "alpha_fe", "alpha_v")}
-    w1, w2 = O.splatting_weights(sd64, flows[:, :, 0].double(), flows[:, :, 1].double())
-    return torch.cat([nhwc(w1), nhwc(w2)], 0)
-
-
-def splat_w_bound(sd, flows):
-    """per-pixel bound of |fp32 - float64| of the splatting weights, (2B, H, W, 1).  The variance term: E[f^2] - E[f]^2 over the 3x3
-    gaussian carries an fp32 rounding e <= 16 * 2^-24 * E[f^2] (nine products and sums, a square, a difference), which moves its square
-    root by at most min(sqrt(e), e / (2 sqrt(d))) - unbounded conditioning where d -> 0; the 1e-9 clamp adds up to 3.2e-5; the weight
-    takes a_v / 2 of the channels' sum.  The consistency term is a bilinear tap and an absolute difference: ~1e-6 * |f| * a_fe."""
-    fl = torch.cat([flows[:, :, 0], flows[:, :, 1]], 0).double()
-    blur = F.conv3d(F.pad(torch.cat([fl ** 2, fl], 1), (1, 1, 1, 1), mode="reflect").unsqueeze(1), sd["g_filter"].double()).squeeze(1)
-    sq, m = torch.split(blur, 2, dim=1)
-    d = (sq - m ** 2).clamp(min=0.0)
-    e = 16 * 2.0 ** -24 * sq
-    dsqrt = torch.minimum(e.sqrt(), e / (2 * d.sqrt()).clamp(min=1e-30)) + 3.2e-5
-    return nhwc(0.5 * float(sd["alpha_v"]) * dsqrt.sum(1, keepdim=True)) + 2e-6 * float(fl.abs().max()) * float(sd["alpha_fe"]) + 1e-6
 
 
 def both(trace, key):
