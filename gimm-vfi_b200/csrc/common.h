@@ -59,7 +59,10 @@ inline TV make_tv(float* p, int n, int h, int w, int c, int ld = 0) {
 struct alignas(16) F4 { float x, y, z, w; };
 GV_HD F4 ld4(const float* p) { return *reinterpret_cast<const F4*>(p); }
 GV_HD void st4(float* p, const F4& v) { *reinterpret_cast<F4*>(p) = v; }
-inline bool vec4_ok(const TV& t) { return (reinterpret_cast<uintptr_t>(t.p) & 15) == 0 && t.c % 4 == 0 && t.ld % 4 == 0 && t.sn % 4 == 0 && !t.f16; }
+inline bool aligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(bytes - 1)) == 0; }
+// t's base, pixel stride and sample stride allow 4-lane vector access (16 bytes fp32, 8 bytes half) at every 4th channel
+inline bool lanes4_ok(const TV& t) { return aligned(t.p, t.f16 ? 8 : 16) && t.ld % 4 == 0 && t.sn % 4 == 0; }
+inline bool vec4_ok(const TV& t) { return lanes4_ok(t) && t.c % 4 == 0 && !t.f16; }
 
 // IEEE binary16 with round-to-nearest-even and saturation to +-65504 (host side, bit exact with cvt.rn.satfinite.f16.f32)
 inline uint16_t gv_f32_to_f16(float f) {
@@ -123,9 +126,26 @@ GV_HD void st4v(const TV& t, int64_t eoff, const F4& v) {
   if (t.f16) { H4 h = {gv_f2h(v.x), gv_f2h(v.y), gv_f2h(v.z), gv_f2h(v.w)}; *reinterpret_cast<H4*>(reinterpret_cast<uint16_t*>(t.p) + eoff) = h; }
   else st4(t.p + eoff, v);
 }
-// like vec4_ok, half tensors allowed (8-byte alignment suffices for them)
-inline bool vec4_ok_any(const TV& t) {
-  return (reinterpret_cast<uintptr_t>(t.p) & (t.f16 ? 7 : 15)) == 0 && t.c % 4 == 0 && t.ld % 4 == 0 && t.sn % 4 == 0;
+// like vec4_ok, half tensors allowed
+inline bool vec4_ok_any(const TV& t) { return lanes4_ok(t) && t.c % 4 == 0; }
+
+// L (1 or 4) consecutive channels as floats.  Any = false: fp32 storage, p[i] or one 16-byte access (ld4 / st4);
+// Any = true: the half-aware ld1 / st1 / ld4v / st4v, which test t.f16 at run time.
+template <int L> GV_HD void ld_lanes(const float* p, float* v) {
+  if constexpr (L == 4) { const F4 a = ld4(p); v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; }
+  else v[0] = p[0];
+}
+template <int L, bool Any> GV_HD void ld_lanes(const TV& t, int64_t eoff, float* v) {
+  if constexpr (!Any) ld_lanes<L>(t.p + eoff, v);
+  else if constexpr (L == 4) { const F4 a = ld4v(t, eoff); v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; }
+  else v[0] = ld1(t, eoff);
+}
+template <int L, bool Any> GV_HD void st_lanes(const TV& t, int64_t eoff, const float* v) {
+  if constexpr (L == 4) {
+    const F4 a = {v[0], v[1], v[2], v[3]};
+    if constexpr (Any) st4v(t, eoff, a); else st4(t.p + eoff, a);
+  } else if constexpr (Any) st1(t, eoff, v[0]);
+  else t.p[eoff] = v[0];
 }
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_LRELU = 2, ACT_PRELU = 3, ACT_SIGMOID = 4, ACT_TANH = 5, ACT_SIN = 6, ACT_GELU = 7 /* exact (erf) GELU: nn.GELU() of the FlowFormer / Twins MLPs */ };
 
@@ -306,6 +326,14 @@ inline void parallel_for(Ctx& cx, int64_t n, const F& f, const char* name) {
   gv_check_launch(name);
   if (cx.prof) cx.prof->end(cx.stream);
 #endif
+}
+
+// A pointwise op written once over L lanes (functor template K<L, Any>, fields initialised from `a`): K<4, Any> over elems / 4
+// items when `four`, else K<1, Any> over elems items, both under the op's kernel name.
+template <template <int, bool> class K, bool Any = false, class... A>
+inline void lanes_for(Ctx& cx, bool four, int64_t elems, const char* name, const A&... a) {
+  if (four) parallel_for(cx, elems / 4, K<4, Any>{a...}, name);
+  else parallel_for(cx, elems, K<1, Any>{a...}, name);
 }
 
 GV_HD bool gv_isfinite(float v) { return fabsf(v) <= 3.402823466e+38f; }  // false for NaN / +-inf

@@ -90,32 +90,21 @@ void nhwc_to_nchw(Ctx& cx, const TV& src, float* dst, int64_t dst_sn, int64_t ds
   parallel_for(cx, src.pixels() * src.c, NhwcToNchwK{src, dst, dst_sn, dst_sc, scale, shift, clamp01}, "nhwc_to_nchw");
 }
 
-struct CopyK {
+// The pointwise ops below with a 4-channel form are functor templates K<L, Any>: L channels per item, Any = half-aware storage
+// (precision mode 4's half tensors).  Each lane's arithmetic is written once; lanes_for picks the width.
+template <int L, bool Any> struct CopyK {
   TV src, dst;
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    dst.p[dst.off(q.n, q.y, q.x) + q.c] = src.p[src.off(q.n, q.y, q.x) + q.c];
-  }
-};
-struct CopyK4 {
-  TV src, dst;
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c / 4);
-    st4(dst.p + dst.off(q.n, q.y, q.x) + q.c * 4, ld4(src.p + src.off(q.n, q.y, q.x) + q.c * 4));
-  }
-};
-struct CopyAnyK {   // either side may be half precision (precision mode 4 concat buffers)
-  TV src, dst;
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    st1(dst, dst.off(q.n, q.y, q.x) + q.c, ld1(src, src.off(q.n, q.y, q.x) + q.c));
+    const Idx4 q = decode4(i, dst.h, dst.w, dst.c / L);
+    float v[L];
+    ld_lanes<L, Any>(src, src.off(q.n, q.y, q.x) + q.c * L, v);
+    st_lanes<L, Any>(dst, dst.off(q.n, q.y, q.x) + q.c * L, v);
   }
 };
 void copy_channels(Ctx& cx, const TV& src, const TV& dst) {
-  if (src.f16 || dst.f16) { parallel_for(cx, dst.pixels() * dst.c, CopyAnyK{src, dst}, "copy_channels"); return; }
+  if (src.f16 || dst.f16) { parallel_for(cx, dst.pixels() * dst.c, CopyK<1, true>{src, dst}, "copy_channels"); return; }
   TV s4 = src; s4.c = dst.c;
-  if (vec4_ok(s4) && vec4_ok(dst)) { parallel_for(cx, dst.pixels() * (dst.c / 4), CopyK4{src, dst}, "copy_channels"); return; }
-  parallel_for(cx, dst.pixels() * dst.c, CopyK{src, dst}, "copy_channels");
+  lanes_for<CopyK>(cx, vec4_ok(s4) && vec4_ok(dst), dst.pixels() * dst.c, "copy_channels", src, dst);
 }
 
 // ---- driver-side pre/post-processing (src/video_Nx.py:40-50,152-153,182-202; src/utils/utils.py:156-185) ----
@@ -177,6 +166,13 @@ GV_HD float fv_sqrt(float a) {
   return __fsqrt_rn(a);
 #else
   return std::sqrt(a);
+#endif
+}
+GV_HD float fv_fma(float a, float b, float c) {   // a * b + c, one rounding on the GPU, two on the host (no contraction there)
+#ifdef __CUDA_ARCH__
+  return __fmaf_rn(a, b, c);
+#else
+  return a * b + c;
 #endif
 }
 GV_HD double fv_dmul(double a, double b) {
@@ -338,85 +334,50 @@ void pad_image4(Ctx& cx, const TV& src, const TV& dst, int pad) {
 
 // reflect-padded copy (padding_mode="reflect"): lets the tensor-core conv, whose TMA can only zero-fill, run the
 // reflect-padded layers (gimmvfi_r.py:94-96,106-108) as a "valid" conv on the padded buffer
-struct PadReflectK {
+template <int L, bool Any> struct PadReflectK {
   TV src, dst; int pad;
-  GV_HD int refl(int v, int n) const { return v < 0 ? -v : (v >= n ? 2 * n - 2 - v : v); }
+  GV_HD static int refl(int v, int n) { return v < 0 ? -v : (v >= n ? 2 * n - 2 - v : v); }
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    int y = refl(q.y - pad, src.h), x = refl(q.x - pad, src.w);
-    dst.p[dst.off(q.n, q.y, q.x) + q.c] = src.p[src.off(q.n, y, x) + q.c];
-  }
-};
-struct PadReflectK4 {
-  TV src, dst; int pad;
-  GV_HD int refl(int v, int n) const { return v < 0 ? -v : (v >= n ? 2 * n - 2 - v : v); }
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c / 4);
-    int y = refl(q.y - pad, src.h), x = refl(q.x - pad, src.w);
-    st4(dst.p + dst.off(q.n, q.y, q.x) + q.c * 4, ld4(src.p + src.off(q.n, y, x) + q.c * 4));
-  }
-};
-struct PadReflectK16 {   // half-precision tensors (2-byte elements)
-  TV src, dst; int pad;
-  GV_HD int refl(int v, int n) const { return v < 0 ? -v : (v >= n ? 2 * n - 2 - v : v); }
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    int y = refl(q.y - pad, src.h), x = refl(q.x - pad, src.w);
-    reinterpret_cast<uint16_t*>(dst.p)[dst.off(q.n, q.y, q.x) + q.c] = reinterpret_cast<const uint16_t*>(src.p)[src.off(q.n, y, x) + q.c];
+    const Idx4 q = decode4(i, dst.h, dst.w, dst.c / L);
+    const int y = refl(q.y - pad, src.h), x = refl(q.x - pad, src.w);
+    float v[L];
+    ld_lanes<L, Any>(src, src.off(q.n, y, x) + q.c * L, v);
+    st_lanes<L, Any>(dst, dst.off(q.n, q.y, q.x) + q.c * L, v);
   }
 };
 void pad_reflect(Ctx& cx, const TV& src, const TV& dst, int pad) {
   if (src.f16 != dst.f16) throw std::runtime_error("pad_reflect: source and destination must have the same storage type");
   if (src.f16) {
     // a pure copy: two half channels are one 32-bit element, so an even-strided half tensor is an fp32 tensor of half the width
-    if (src.c % 8 == 0 && src.ld % 8 == 0 && dst.ld % 8 == 0 && src.sn % 8 == 0 && dst.sn % 8 == 0 &&
-        (reinterpret_cast<uintptr_t>(src.p) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst.p) & 15) == 0) {
-      TV s2 = src, d2 = dst;
-      s2.f16 = d2.f16 = 0; s2.c /= 2; d2.c /= 2; s2.ld /= 2; d2.ld /= 2; s2.sn /= 2; d2.sn /= 2;
-      parallel_for(cx, d2.pixels() * (d2.c / 4), PadReflectK4{s2, d2, pad}, "pad_reflect");
-      return;
-    }
-    parallel_for(cx, dst.pixels() * dst.c, PadReflectK16{src, dst, pad}, "pad_reflect"); return;
+    auto even = [](const TV& t) { return t.c % 2 == 0 && t.ld % 2 == 0 && t.sn % 2 == 0; };
+    auto pairs = [](TV t) { t.f16 = 0; t.c /= 2; t.ld /= 2; t.sn /= 2; return t; };
+    const TV s2 = pairs(src), d2 = pairs(dst);
+    if (even(src) && even(dst) && vec4_ok(s2) && vec4_ok(d2)) parallel_for(cx, d2.pixels() * (d2.c / 4), PadReflectK<4, false>{s2, d2, pad}, "pad_reflect");
+    else parallel_for(cx, dst.pixels() * dst.c, PadReflectK<1, true>{src, dst, pad}, "pad_reflect");
+    return;
   }
-  if (vec4_ok(src) && vec4_ok(dst)) { parallel_for(cx, dst.pixels() * (dst.c / 4), PadReflectK4{src, dst, pad}, "pad_reflect"); return; }
-  parallel_for(cx, dst.pixels() * dst.c, PadReflectK{src, dst, pad}, "pad_reflect");
+  lanes_for<PadReflectK>(cx, vec4_ok(src) && vec4_ok(dst), dst.pixels() * dst.c, "pad_reflect", src, dst, pad);
 }
 
 // zero-padded copy: dst (n, h+2p, w+2p) gets src's channels in its interior, zeros elsewhere (all dst.ld lanes)
-struct PadZeroK {
+template <int L, bool Any> struct PadZeroK {
   TV src, dst; int pad;
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.ld);
-    int y = q.y - pad, x = q.x - pad;
-    float v = 0.f;
-    if (q.c < src.c && y >= 0 && y < src.h && x >= 0 && x < src.w) v = src.p[src.off(q.n, y, x) + q.c];
-    dst.p[dst.off(q.n, q.y, q.x) + q.c] = v;
-  }
-};
-struct PadZeroK4 {   // 4 lanes per thread (16-byte loads / stores); lanes >= src.c are written as zeros like PadZeroK does
-  TV src, dst; int pad;
-  GV_HD void operator()(int64_t i) const {
-    const int g4 = dst.ld >> 2;
-    const int g = (int)(i % g4); int64_t r = i / g4;
-    const int px = (int)(r % dst.w); r /= dst.w; const int py = (int)(r % dst.h); const int n = (int)(r / dst.h);
-    const int y = py - pad, x = px - pad, c0 = g * 4;
-    F4 v = {0.f, 0.f, 0.f, 0.f};
+    const Idx4 q = decode4(i, dst.h, dst.w, dst.ld / L);
+    const int y = q.y - pad, x = q.x - pad, c0 = q.c * L;
+    float v[L];
+    for (int k = 0; k < L; ++k) v[k] = 0.f;
     if (c0 < src.c && y >= 0 && y < src.h && x >= 0 && x < src.w) {
-      v = ld4(src.p + src.off(n, y, x) + c0);   // (c0 + 3 < src.ld: both pixel strides are multiples of 4)
-      if (c0 + 1 >= src.c) v.y = 0.f;
-      if (c0 + 2 >= src.c) v.z = 0.f;
-      if (c0 + 3 >= src.c) v.w = 0.f;
+      ld_lanes<L, Any>(src, src.off(q.n, y, x) + c0, v);   // (c0 + L - 1 < src.ld: the 4-lane form needs ((src.c + 3) & ~3) <= src.ld)
+      for (int k = 1; k < L; ++k)
+        if (c0 + k >= src.c) v[k] = 0.f;
     }
-    st4(dst.p + dst.off(n, py, px) + c0, v);
+    st_lanes<L, Any>(dst, dst.off(q.n, q.y, q.x) + c0, v);
   }
 };
 void pad_zero(Ctx& cx, const TV& src, const TV& dst, int pad) {
-  auto al16 = [](const TV& t) { return (reinterpret_cast<uintptr_t>(t.p) & 15) == 0 && t.ld % 4 == 0 && t.sn % 4 == 0 && !t.f16; };
-  if (al16(src) && al16(dst) && ((src.c + 3) & ~3) <= src.ld) {
-    parallel_for(cx, dst.pixels() * (dst.ld / 4), PadZeroK4{src, dst, pad}, "pad_zero");
-    return;
-  }
-  parallel_for(cx, dst.pixels() * dst.ld, PadZeroK{src, dst, pad}, "pad_zero");
+  const bool four = lanes4_ok(src) && lanes4_ok(dst) && !src.f16 && !dst.f16 && ((src.c + 3) & ~3) <= src.ld;
+  lanes_for<PadZeroK>(cx, four, dst.pixels() * dst.ld, "pad_zero", src, dst, pad);
 }
 
 struct FillK {
@@ -444,10 +405,10 @@ void axpby(Ctx& cx, const TV& a, float alpha, const TV& b, float beta, const TV&
 // ------------------------------------------------------------------ resize
 // F.interpolate(mode="bilinear", align_corners=False) — modules/fi_utils.py:67-70.
 // src coordinate = rscale * (dst + 0.5) - 0.5 clamped at 0 (ATen area_pixel_compute_source_index).
-struct ResizeK {
+template <int L, bool Any> struct ResizeK {
   TV src, dst; float rsy, rsx, mult; int accumulate, act;
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
+    const Idx4 q = decode4(i, dst.h, dst.w, dst.c / L);
     float sy = rsy * ((float)q.y + 0.5f) - 0.5f; if (sy < 0.f) sy = 0.f;
     float sx = rsx * ((float)q.x + 0.5f) - 0.5f; if (sx < 0.f) sx = 0.f;
     int y0 = (int)sy, x0 = (int)sx;
@@ -456,47 +417,30 @@ struct ResizeK {
     int y1 = y0 + (y0 < src.h - 1 ? 1 : 0), x1 = x0 + (x0 < src.w - 1 ? 1 : 0);
     float ly1 = sy - (float)y0, lx1 = sx - (float)x0;
     float ly0 = 1.f - ly1, lx0 = 1.f - lx1;
-    const float* b = src.p + (int64_t)q.n * src.sn + q.c;
-    float v00 = b[((int64_t)y0 * src.w + x0) * src.ld], v01 = b[((int64_t)y0 * src.w + x1) * src.ld];
-    float v10 = b[((int64_t)y1 * src.w + x0) * src.ld], v11 = b[((int64_t)y1 * src.w + x1) * src.ld];
-    float v = ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
-    v *= mult;
-    if (act == ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
-    float* o = dst.p + dst.off(q.n, q.y, q.x) + q.c;
-    *o = accumulate ? (*o + v) : v;
+    const int64_t b = (int64_t)q.n * src.sn + q.c * L;
+    float v00[L], v01[L], v10[L], v11[L];
+    ld_lanes<L, Any>(src, b + ((int64_t)y0 * src.w + x0) * src.ld, v00); ld_lanes<L, Any>(src, b + ((int64_t)y0 * src.w + x1) * src.ld, v01);
+    ld_lanes<L, Any>(src, b + ((int64_t)y1 * src.w + x0) * src.ld, v10); ld_lanes<L, Any>(src, b + ((int64_t)y1 * src.w + x1) * src.ld, v11);
+    const int64_t o = dst.off(q.n, q.y, q.x) + q.c * L;
+    float old[L];
+    if (accumulate) ld_lanes<L, Any>(dst, o, old);
+    float r[L];
+    for (int k = 0; k < L; ++k) {
+      // ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11) with the GPU's FMA contraction spelled out (the lx1 and ly0
+      // terms fused), as both widths have always computed it: nvcc may fuse either product of a sum, and left alone it chose
+      // differently for the two widths
+      const float r0 = fv_fma(lx1, v01[k], fv_mul(lx0, v00[k])), r1 = fv_fma(lx1, v11[k], fv_mul(lx0, v10[k]));
+      float v = fv_fma(ly0, r0, fv_mul(ly1, r1));
+      v = fv_mul(v, mult);
+      if (act == ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
+      r[k] = accumulate ? (old[k] + v) : v;
+    }
+    st_lanes<L, Any>(dst, o, r);
   }
 };
-struct ResizeK4 {   // 4 channels per thread, the per-component arithmetic of ResizeK unchanged
-  TV src, dst; float rsy, rsx, mult; int accumulate, act;
-  GV_HD float fin(float v00, float v01, float v10, float v11, float lx0, float lx1, float ly0, float ly1, float old) const {
-    float v = ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
-    v *= mult;
-    if (act == ACT_SIGMOID) v = 1.f / (1.f + expf(-v));
-    return accumulate ? (old + v) : v;
-  }
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c / 4);
-    float sy = rsy * ((float)q.y + 0.5f) - 0.5f; if (sy < 0.f) sy = 0.f;
-    float sx = rsx * ((float)q.x + 0.5f) - 0.5f; if (sx < 0.f) sx = 0.f;
-    int y0 = (int)sy, x0 = (int)sx;
-    if (y0 > src.h - 1) y0 = src.h - 1;
-    if (x0 > src.w - 1) x0 = src.w - 1;
-    int y1 = y0 + (y0 < src.h - 1 ? 1 : 0), x1 = x0 + (x0 < src.w - 1 ? 1 : 0);
-    float ly1 = sy - (float)y0, lx1 = sx - (float)x0;
-    float ly0 = 1.f - ly1, lx0 = 1.f - lx1;
-    const float* b = src.p + (int64_t)q.n * src.sn + q.c * 4;
-    const F4 a00 = ld4(b + ((int64_t)y0 * src.w + x0) * src.ld), a01 = ld4(b + ((int64_t)y0 * src.w + x1) * src.ld);
-    const F4 a10 = ld4(b + ((int64_t)y1 * src.w + x0) * src.ld), a11 = ld4(b + ((int64_t)y1 * src.w + x1) * src.ld);
-    float* o = dst.p + dst.off(q.n, q.y, q.x) + q.c * 4;
-    F4 old = {0.f, 0.f, 0.f, 0.f};
-    if (accumulate) old = ld4(o);
-    F4 r;
-    r.x = fin(a00.x, a01.x, a10.x, a11.x, lx0, lx1, ly0, ly1, old.x); r.y = fin(a00.y, a01.y, a10.y, a11.y, lx0, lx1, ly0, ly1, old.y);
-    r.z = fin(a00.z, a01.z, a10.z, a11.z, lx0, lx1, ly0, ly1, old.z); r.w = fin(a00.w, a01.w, a10.w, a11.w, lx0, lx1, ly0, ly1, old.w);
-    st4(o, r);
-  }
-};
-struct ResizeAnyK4 {   // ResizeK4 with half-aware loads / stores (no accumulate mode)
+// The half-aware form (precision mode 4's concat buffers): the same arithmetic, kept as its own functor because the ResizeK<4, true>
+// instance of the template above compiled to a different load schedule that measured slower on the full-resolution 4K concat
+struct ResizeAnyK4 {
   TV src, dst; float rsy, rsx, mult; int act;
   GV_HD float fin(float v00, float v01, float v10, float v11, float lx0, float lx1, float ly0, float ly1) const {
     float v = ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
@@ -524,93 +468,43 @@ struct ResizeAnyK4 {   // ResizeK4 with half-aware loads / stores (no accumulate
   }
 };
 void resize_bilinear(Ctx& cx, const TV& src, const TV& dst, float rscale_y, float rscale_x, float mult, int accumulate, int act) {
+  TV s4 = src; s4.c = dst.c;
   if (src.f16 || dst.f16) {
-    TV s4 = src; s4.c = dst.c;
     if (accumulate || !vec4_ok_any(s4) || !vec4_ok_any(dst)) throw std::runtime_error("resize_bilinear: half-precision tensors need 4-channel-aligned views and no accumulation");
     parallel_for(cx, dst.pixels() * (dst.c / 4), ResizeAnyK4{src, dst, rscale_y, rscale_x, mult, act}, "resize_bilinear");
     return;
   }
-  {
-    TV s4 = src; s4.c = dst.c;
-    if (vec4_ok(s4) && vec4_ok(dst)) {
-      parallel_for(cx, dst.pixels() * (dst.c / 4), ResizeK4{src, dst, rscale_y, rscale_x, mult, accumulate, act}, "resize_bilinear");
-      return;
-    }
-  }
-  parallel_for(cx, dst.pixels() * dst.c, ResizeK{src, dst, rscale_y, rscale_x, mult, accumulate, act}, "resize_bilinear");
+  lanes_for<ResizeK>(cx, vec4_ok(s4) && vec4_ok(dst), dst.pixels() * dst.c, "resize_bilinear", src, dst, rscale_y, rscale_x, mult, accumulate, act);
 }
 
 // ---------------------------------------------------------------- backwarp
-// modules/fi_utils.py:19-49.
-struct BackwarpK {
+// modules/fi_utils.py:19-49.  The four corners in tap_fetch's order and products.
+template <int L, bool Any> struct BackwarpK {
   TV src, flow, dst;
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    const float* f = flow.p + flow.off(q.n, q.y, q.x);
-    BilinearTap t = border_tap(q.x, q.y, f[0], f[1], flow.w, flow.h, src.w, src.h);
-    dst.p[dst.off(q.n, q.y, q.x) + q.c] = tap_fetch(src, q.n, t, q.c);
+  GV_HD void corner(float* v, int64_t eoff, float w) const {
+    float a[L];
+    ld_lanes<L, Any>(src, eoff, a);
+    for (int k = 0; k < L; ++k) v[k] += a[k] * w;
   }
-};
-struct BackwarpK4 {   // 4 channels per thread; same tap order / products as tap_fetch
-  TV src, flow, dst;
-  GV_HD void acc(F4& v, const float* p, float w) const { const F4 a = ld4(p); v.x += a.x * w; v.y += a.y * w; v.z += a.z * w; v.w += a.w * w; }
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c / 4);
+    const Idx4 q = decode4(i, dst.h, dst.w, dst.c / L);
     const float* f = flow.p + flow.off(q.n, q.y, q.x);
     const BilinearTap t = border_tap(q.x, q.y, f[0], f[1], flow.w, flow.h, src.w, src.h);
-    const float* b = src.p + (int64_t)q.n * src.sn + q.c * 4;
-    F4 v = {0.f, 0.f, 0.f, 0.f};
-    if (t.vy0 && t.vx0) acc(v, b + ((int64_t)t.y0 * src.w + t.x0) * src.ld, t.wx0 * t.wy0);
-    if (t.vy0 && t.vx1) acc(v, b + ((int64_t)t.y0 * src.w + t.x1) * src.ld, t.wx1 * t.wy0);
-    if (t.vy1 && t.vx0) acc(v, b + ((int64_t)t.y1 * src.w + t.x0) * src.ld, t.wx0 * t.wy1);
-    if (t.vy1 && t.vx1) acc(v, b + ((int64_t)t.y1 * src.w + t.x1) * src.ld, t.wx1 * t.wy1);
-    st4(dst.p + dst.off(q.n, q.y, q.x) + q.c * 4, v);
-  }
-};
-struct BackwarpAnyK4 {   // BackwarpK4 with half-aware loads / stores
-  TV src, flow, dst;
-  GV_HD void acc(F4& v, int64_t eoff, float w) const { const F4 a = ld4v(src, eoff); v.x += a.x * w; v.y += a.y * w; v.z += a.z * w; v.w += a.w * w; }
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c / 4);
-    const float* f = flow.p + flow.off(q.n, q.y, q.x);
-    const BilinearTap t = border_tap(q.x, q.y, f[0], f[1], flow.w, flow.h, src.w, src.h);
-    const int64_t b = (int64_t)q.n * src.sn + q.c * 4;
-    F4 v = {0.f, 0.f, 0.f, 0.f};
-    if (t.vy0 && t.vx0) acc(v, b + ((int64_t)t.y0 * src.w + t.x0) * src.ld, t.wx0 * t.wy0);
-    if (t.vy0 && t.vx1) acc(v, b + ((int64_t)t.y0 * src.w + t.x1) * src.ld, t.wx1 * t.wy0);
-    if (t.vy1 && t.vx0) acc(v, b + ((int64_t)t.y1 * src.w + t.x0) * src.ld, t.wx0 * t.wy1);
-    if (t.vy1 && t.vx1) acc(v, b + ((int64_t)t.y1 * src.w + t.x1) * src.ld, t.wx1 * t.wy1);
-    st4v(dst, dst.off(q.n, q.y, q.x) + q.c * 4, v);
-  }
-};
-struct BackwarpAnyK {   // scalar: 3-channel image warps into a half-precision concat buffer
-  TV src, flow, dst;
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, dst.h, dst.w, dst.c);
-    const float* f = flow.p + flow.off(q.n, q.y, q.x);
-    const BilinearTap t = border_tap(q.x, q.y, f[0], f[1], flow.w, flow.h, src.w, src.h);
-    const int64_t b = (int64_t)q.n * src.sn + q.c;
-    float v = 0.f;
-    if (t.vy0 && t.vx0) v += ld1(src, b + ((int64_t)t.y0 * src.w + t.x0) * src.ld) * (t.wx0 * t.wy0);
-    if (t.vy0 && t.vx1) v += ld1(src, b + ((int64_t)t.y0 * src.w + t.x1) * src.ld) * (t.wx1 * t.wy0);
-    if (t.vy1 && t.vx0) v += ld1(src, b + ((int64_t)t.y1 * src.w + t.x0) * src.ld) * (t.wx0 * t.wy1);
-    if (t.vy1 && t.vx1) v += ld1(src, b + ((int64_t)t.y1 * src.w + t.x1) * src.ld) * (t.wx1 * t.wy1);
-    st1(dst, dst.off(q.n, q.y, q.x) + q.c, v);
+    const int64_t b = (int64_t)q.n * src.sn + q.c * L;
+    float v[L];
+    for (int k = 0; k < L; ++k) v[k] = 0.f;
+    if (t.vy0 && t.vx0) corner(v, b + ((int64_t)t.y0 * src.w + t.x0) * src.ld, t.wx0 * t.wy0);
+    if (t.vy0 && t.vx1) corner(v, b + ((int64_t)t.y0 * src.w + t.x1) * src.ld, t.wx1 * t.wy0);
+    if (t.vy1 && t.vx0) corner(v, b + ((int64_t)t.y1 * src.w + t.x0) * src.ld, t.wx0 * t.wy1);
+    if (t.vy1 && t.vx1) corner(v, b + ((int64_t)t.y1 * src.w + t.x1) * src.ld, t.wx1 * t.wy1);
+    st_lanes<L, Any>(dst, dst.off(q.n, q.y, q.x) + q.c * L, v);
   }
 };
 void backwarp(Ctx& cx, const TV& src, const TV& flow, const TV& dst) {
   if (flow.f16) throw std::runtime_error("backwarp: the flow field must be fp32");
-  if (src.f16 || dst.f16) {
-    TV s4 = src; s4.c = dst.c;
-    if (vec4_ok_any(s4) && vec4_ok_any(dst)) parallel_for(cx, dst.pixels() * (dst.c / 4), BackwarpAnyK4{src, flow, dst}, "backwarp");
-    else parallel_for(cx, dst.pixels() * dst.c, BackwarpAnyK{src, flow, dst}, "backwarp");
-    return;
-  }
-  {
-    TV s4 = src; s4.c = dst.c;
-    if (vec4_ok(s4) && vec4_ok(dst)) { parallel_for(cx, dst.pixels() * (dst.c / 4), BackwarpK4{src, flow, dst}, "backwarp"); return; }
-  }
-  parallel_for(cx, dst.pixels() * dst.c, BackwarpK{src, flow, dst}, "backwarp");
+  TV s4 = src; s4.c = dst.c;
+  if (src.f16 || dst.f16) lanes_for<BackwarpK, true>(cx, vec4_ok_any(s4) && vec4_ok_any(dst), dst.pixels() * dst.c, "backwarp", src, flow, dst);
+  else lanes_for<BackwarpK>(cx, vec4_ok(s4) && vec4_ok(dst), dst.pixels() * dst.c, "backwarp", src, flow, dst);
 }
 
 // ----------------------------------------------------------- pixel shuffle
@@ -688,46 +582,29 @@ void instnorm_stats(Ctx& cx, const TV& x, float* mean_rstd, float* scratch, int6
   parallel_for(cx, (int64_t)x.n * 32 * x.c, InFoldK{part, fold, x.c, chunks}, "instnorm_fold");
   parallel_for(cx, (int64_t)x.n * x.c, InFinalK{fold, mean_rstd, x.c, 1.0 / ((double)x.h * x.w)}, "instnorm_final");
 }
-struct InApplyK {
+template <int L, bool Any> struct InApplyK {
   TV x, res, out; const float* mr; int act1, act2;
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, out.h, out.w, out.c);
-    const float* s = mr + ((int64_t)q.n * x.c + q.c) * 2;
-    float v = (x.p[x.off(q.n, q.y, q.x) + q.c] - s[0]) * s[1];
-    v = apply_act(v, act1, nullptr, 0);
-    if (res.p) v += res.p[res.off(q.n, q.y, q.x) + q.c];
-    v = apply_act(v, act2, nullptr, 0);
-    out.p[out.off(q.n, q.y, q.x) + q.c] = v;
-  }
-};
-struct InApplyK4 {
-  TV x, res, out; const float* mr; int act1, act2;
-  GV_HD float one(float xv, float m, float r, float rv) const {
-    float v = (xv - m) * r;
-    v = apply_act(v, act1, nullptr, 0);
-    if (res.p) v += rv;
-    return apply_act(v, act2, nullptr, 0);
-  }
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, out.h, out.w, out.c / 4);
-    const int c = q.c * 4;
-    const float* s = mr + ((int64_t)q.n * x.c + c) * 2;   // (mean, rstd) pairs of 4 consecutive channels
-    const F4 s01 = ld4(s), s23 = ld4(s + 4);
-    const F4 a = ld4(x.p + x.off(q.n, q.y, q.x) + c);
-    F4 rv = {0.f, 0.f, 0.f, 0.f};
-    if (res.p) rv = ld4(res.p + res.off(q.n, q.y, q.x) + c);
-    F4 o;
-    o.x = one(a.x, s01.x, s01.y, rv.x); o.y = one(a.y, s01.z, s01.w, rv.y);
-    o.z = one(a.z, s23.x, s23.y, rv.z); o.w = one(a.w, s23.z, s23.w, rv.w);
-    st4(out.p + out.off(q.n, q.y, q.x) + c, o);
+    const Idx4 q = decode4(i, out.h, out.w, out.c / L);
+    const int c = q.c * L;
+    const float* s = mr + ((int64_t)q.n * x.c + c) * 2;
+    float sm[2 * L];   // (mean, rstd) pairs of the L channels
+    ld_lanes<L>(s, sm); ld_lanes<L>(s + L, sm + L);
+    float a[L], rv[L], o[L];
+    ld_lanes<L, Any>(x, x.off(q.n, q.y, q.x) + c, a);
+    if (res.p) ld_lanes<L, Any>(res, res.off(q.n, q.y, q.x) + c, rv);
+    for (int k = 0; k < L; ++k) {
+      float v = (a[k] - sm[2 * k]) * sm[2 * k + 1];
+      v = apply_act(v, act1, nullptr, 0);
+      if (res.p) v += rv[k];
+      o[k] = apply_act(v, act2, nullptr, 0);
+    }
+    st_lanes<L, Any>(out, out.off(q.n, q.y, q.x) + c, o);
   }
 };
 void instnorm_apply(Ctx& cx, const TV& x, const float* mean_rstd, int act1, const TV& res, int act2, const TV& out) {
-  if (vec4_ok(x) && vec4_ok(out) && (!res.p || vec4_ok(res)) && (reinterpret_cast<uintptr_t>(mean_rstd) & 15) == 0 && x.c == out.c) {
-    parallel_for(cx, out.pixels() * (out.c / 4), InApplyK4{x, res, out, mean_rstd, act1, act2}, "instnorm_apply");
-    return;
-  }
-  parallel_for(cx, out.pixels() * out.c, InApplyK{x, res, out, mean_rstd, act1, act2}, "instnorm_apply");
+  const bool four = vec4_ok(x) && vec4_ok(out) && (!res.p || vec4_ok(res)) && aligned(mean_rstd, 16) && x.c == out.c;
+  lanes_for<InApplyK>(cx, four, out.pixels() * out.c, "instnorm_apply", x, res, out, mean_rstd, act1, act2);
 }
 
 // ------------------------------------------------------- flow normalisation
@@ -985,18 +862,6 @@ __global__ void __launch_bounds__(256) softsplat_acc_v4_kernel(TV lat, TV flow, 
     }
   }
 }
-// "zeroeps" normalisation, 4 channels per thread
-struct SplatNormK4 {
-  TV acc, out;
-  GV_HD void operator()(int64_t i) const {
-    const int g = (int)(i & 3); int64_t r = i >> 2;
-    const int x = (int)(r % out.w); r /= out.w; const int y = (int)(r % out.h); const int n = (int)(r / out.h);
-    const float* a = acc.p + acc.off(n, y, x);
-    float d = a[16]; if (d == 0.f) d = 1.f;
-    const F4 v = ld4(a + 4 * g);
-    st4(out.p + out.off(n, y, x) + 4 * g, F4{v.x / d, v.y / d, v.z / d, v.w / d});
-  }
-};
 #endif
 
 #ifndef GV_HOSTSIM
@@ -1112,23 +977,21 @@ void softsplat_accumulate(Ctx& cx, const TV& lat, const TV& flow, const TV& metr
   parallel_for(cx, lat.pixels() * 17, SplatAccK{lat, flow, metric, acc, t_per_sample, t_mode}, "softsplat_accumulate");
 }
 // "zeroeps" normalisation, modules/softsplat.py:330-344.
-struct SplatNormK {
+template <int L, bool Any> struct SplatNormK {
   TV acc, out;
   GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, out.h, out.w, 16);
+    const Idx4 q = decode4(i, out.h, out.w, 16 / L);
     const float* a = acc.p + acc.off(q.n, q.y, q.x);
     float d = a[16]; if (d == 0.f) d = 1.f;
-    out.p[out.off(q.n, q.y, q.x) + q.c] = a[q.c] / d;
+    float v[L];
+    ld_lanes<L>(a + q.c * L, v);
+    for (int k = 0; k < L; ++k) v[k] = v[k] / d;
+    st_lanes<L, Any>(out, out.off(q.n, q.y, q.x) + q.c * L, v);
   }
 };
 void softsplat_normalize(Ctx& cx, const TV& acc, const TV& out) {
-#ifndef GV_HOSTSIM
-  if (out.c == 16 && vec4_ok(out) && (reinterpret_cast<uintptr_t>(acc.p) & 15) == 0 && acc.ld % 4 == 0 && acc.sn % 4 == 0) {
-    parallel_for(cx, out.pixels() * 4, SplatNormK4{acc, out}, "softsplat_normalize");
-    return;
-  }
-#endif
-  parallel_for(cx, out.pixels() * 16, SplatNormK{acc, out}, "softsplat_normalize");
+  const bool four = out.c == 16 && vec4_ok(out) && lanes4_ok(acc) && !acc.f16;
+  lanes_for<SplatNormK>(cx, four, out.pixels() * 16, "softsplat_normalize", acc, out);
 }
 
 // ------------------------------------------------- differentiable splat (training)
@@ -1369,29 +1232,10 @@ void warp_blend(Ctx& cx, const TV& img0, const TV& img1, const TV& f0, const TV&
   parallel_for(cx, out.pixels() * 3, WarpBlendK{img0, img1, f0, f1, mask, out}, "warp_blend");
 }
 
-// multi_flow_combine, fi_components.py:57-88: 3 x (2 warps, blend, + residual) and their mean.
+// multi_flow_combine, fi_components.py:57-88: 3 x (2 warps, blend, + residual) and their mean.  One thread per pixel: the taps are
+// computed once per flow pair, the four corners of each frame are fetched as 16-byte pixels (3 colours + padding lane), the nine blended
+// values leave as three 16-byte stores.  Per value, tap_fetch's corner order and products.
 struct MultiFlowBlendK {
-  TV i0, i1, f0, f1, m, res, w9, mean3;
-  GV_HD void operator()(int64_t i) const {
-    Idx4 q = decode4(i, w9.h, w9.w, 3);
-    float acc = 0.f;
-    for (int k = 0; k < 3; ++k) {
-      const float* a = f0.p + f0.off(q.n, q.y, q.x) + 2 * k; const float* b = f1.p + f1.off(q.n, q.y, q.x) + 2 * k;
-      BilinearTap t0 = border_tap(q.x, q.y, a[0], a[1], f0.w, f0.h, i0.w, i0.h);
-      BilinearTap t1 = border_tap(q.x, q.y, b[0], b[1], f1.w, f1.h, i1.w, i1.h);
-      float mm = m.p[m.off(q.n, q.y, q.x) + k];
-      float v = mm * tap_fetch(i0, q.n, t0, q.c) + (1.f - mm) * tap_fetch(i1, q.n, t1, q.c);
-      v += res.p[res.off(q.n, q.y, q.x) + 3 * k + q.c];
-      w9.p[w9.off(q.n, q.y, q.x) + 3 * k + q.c] = v;
-      acc += v;
-    }
-    mean3.p[mean3.off(q.n, q.y, q.x) + q.c] = acc / 3.f;
-  }
-};
-// One thread per PIXEL (the form above runs one per (pixel, colour): every thread re-derives the three bilinear taps of both frames and
-// re-reads both flow triples): the taps are computed once per flow pair, the four corners of each frame are fetched as 16-byte pixels
-// (3 colours + padding lane), the nine blended values leave as three 16-byte stores.  Same arithmetic and summation order per value.
-struct MultiFlowBlendPxK {
   TV i0, i1, f0, f1, m, res, w9, mean3;
   GV_HD static void fetch3(const TV& s, int n, const BilinearTap& t, float* v) {
     const float* b = s.p + (int64_t)n * s.sn;
@@ -1429,13 +1273,10 @@ struct MultiFlowBlendPxK {
 };
 void multi_flow_blend(Ctx& cx, const TV& img0, const TV& img1, const TV& f0, const TV& f1, const TV& mask, const TV& res,
                       const TV& warps9, const TV& mean3) {
-  auto al16 = [](const TV& t) { return (reinterpret_cast<uintptr_t>(t.p) & 15) == 0 && t.ld % 4 == 0 && t.sn % 4 == 0 && !t.f16; };
-  if (al16(img0) && al16(img1) && img0.ld >= 4 && img1.ld >= 4 && al16(warps9) && warps9.ld >= 12 && al16(mean3) && mean3.ld >= 4 && !f0.f16 && !f1.f16 &&
-      !mask.f16 && !res.f16) {
-    parallel_for(cx, warps9.pixels(), MultiFlowBlendPxK{img0, img1, f0, f1, mask, res, warps9, mean3}, "multi_flow_blend");
-    return;
-  }
-  parallel_for(cx, warps9.pixels() * 3, MultiFlowBlendK{img0, img1, f0, f1, mask, res, warps9, mean3}, "multi_flow_blend");
+  auto px4 = [](const TV& t, int lanes) { return lanes4_ok(t) && !t.f16 && t.ld >= lanes; };
+  if (!px4(img0, 4) || !px4(img1, 4) || !px4(warps9, 12) || !px4(mean3, 4) || f0.f16 || f1.f16 || mask.f16 || res.f16)
+    throw std::runtime_error("multi_flow_blend: frames, warps and mean need 16-byte-aligned fp32 pixels of 4 / 12 / 4 lanes, flows / mask / residual fp32");
+  parallel_for(cx, warps9.pixels(), MultiFlowBlendK{img0, img1, f0, f1, mask, res, warps9, mean3}, "multi_flow_blend");
 }
 
 // fi_components.py:89-92 + gimmvfi_r.py:308: clamp((mean + comb + 1)/2, 0, 1) -> NCHW

@@ -20,34 +20,23 @@ GV_HD float pe_value(int c, int dim, float X, float Y) {
 // ------------------------------------------------------------------ space to depth
 // dst[n, y, x, (ky*k + kx)*C + c] = src[n, y*k + ky, x*k + kx, c]: a k x k stride-k convolution (Twins PatchEmbed twins.py:1122-1149,
 // the sub-sampling convs of GlobalSubSampleAttn twins.py:890-893 / :452-456) becomes a 1x1 convolution over k*k*C channels.
-struct PatchifyK {
+template <int L, bool Any> struct PatchifyK {   // L channels per item
   TV src, dst; int k;
   GV_HD void operator()(int64_t i) const {
-    const int C = src.c, K = k * k * C;
-    const int ch = (int)(i % K); int64_t r = i / K;
+    const int CL = src.c / L, KL = k * k * CL;
+    const int ch = (int)(i % KL); int64_t r = i / KL;
     const int x = (int)(r % dst.w); r /= dst.w; const int y = (int)(r % dst.h); const int n = (int)(r / dst.h);
-    const int t = ch / C, c = ch - t * C, ky = t / k, kx = t - ky * k;
+    const int t = ch / CL, c = (ch - t * CL) * L, ky = t / k, kx = t - ky * k;
     const int sy = y * k + ky, sx = x * k + kx;
-    dst.p[dst.off(n, y, x) + ch] = (sy < src.h && sx < src.w) ? src.p[src.off(n, sy, sx) + c] : 0.f;
-  }
-};
-struct PatchifyK4 {   // 4 channels per thread (C % 4 == 0, 16-byte aligned views)
-  TV src, dst; int k;
-  GV_HD void operator()(int64_t i) const {
-    const int C4 = src.c >> 2, K4 = k * k * C4;
-    const int ch = (int)(i % K4); int64_t r = i / K4;
-    const int x = (int)(r % dst.w); r /= dst.w; const int y = (int)(r % dst.h); const int n = (int)(r / dst.h);
-    const int t = ch / C4, c = (ch - t * C4) * 4, ky = t / k, kx = t - ky * k;
-    const int sy = y * k + ky, sx = x * k + kx;
-    F4 v = {0.f, 0.f, 0.f, 0.f};
-    if (sy < src.h && sx < src.w) v = ld4(src.p + src.off(n, sy, sx) + c);
-    st4(dst.p + dst.off(n, y, x) + t * src.c + c, v);
+    float v[L];
+    for (int j = 0; j < L; ++j) v[j] = 0.f;
+    if (sy < src.h && sx < src.w) ld_lanes<L, Any>(src, src.off(n, sy, sx) + c, v);
+    st_lanes<L, Any>(dst, dst.off(n, y, x) + t * src.c + c, v);
   }
 };
 void patchify(Ctx& cx, const TV& src, const TV& dst, int k) {
   if (dst.c != k * k * src.c || dst.n != src.n) throw std::runtime_error("patchify: shape mismatch");
-  if (vec4_ok(src) && vec4_ok(dst)) parallel_for(cx, dst.pixels() * (dst.c / 4), PatchifyK4{src, dst, k}, "patchify");
-  else parallel_for(cx, dst.pixels() * dst.c, PatchifyK{src, dst, k}, "patchify");
+  lanes_for<PatchifyK>(cx, vec4_ok(src) && vec4_ok(dst), dst.pixels() * dst.c, "patchify", src, dst, k);
 }
 
 // ------------------------------------------------------------------ LayerNorm
