@@ -988,7 +988,9 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
       for (int p = 0; p < S; ++p) { copy_channels(cx, z.batch(slot[src[p]], 1), Pzr[s].batch(p, 1)); copy_channels(cx, q.batch(slot[src[p]], 1), Pq[s].batch(p, 1)); }
       A.release(mk);
     }
+  tap_copy(cx, "raft.cnet", hx.slice(0, 256));   // tanh(net) | relu(inp) in pair order (the GRU overwrites net in place)
   for (int it = 0; it < r.iters; ++it) {
+    if (debug_ && it == r.iters - 1) { tap_copy(cx, "raft.coords_last", coords1); tap_copy(cx, "raft.net_last", hcur); }
     if (raft_direct) {   // each run's sources against its targets' features (GIMM-VFI-R: frame 1's for direction 0 and vice versa)
       for (const auto& run : runs)
         corr_lookup_direct(cx, fmap.batch(src[run.first], run.second), rfeat_of(tgt[run.first]), coords1.batch(run.first, run.second),
@@ -999,12 +1001,14 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
     coords_minus_grid(cx, coords1, flow, hx.slice(382, 2));
     // (a copy: every later iteration's lookup overwrites `corr`)
     if (it == 0 && debug_) { TV snap = A.tensor(S, h, w, 324); copy_channels(cx, corr, snap); tap("raft.corr_it0", snap); }
+    if (debug_ && it == r.iters - 1) tap_copy(cx, "raft.corr_last", corr);
     // BasicMotionEncoder raft/update.py:94-112
     N.conv(u + ".encoder.convc1", corr, cor1, ACT_RELU);
     N.conv(u + ".encoder.convc2", cor1, corflo.slice(0, 192), ACT_RELU);
     N.conv7x(u + ".encoder.convf1", flow, flo1, ACT_RELU);
     N.conv(u + ".encoder.convf2", flo1, corflo.slice(192, 64), ACT_RELU);
     N.conv(u + ".encoder.conv", corflo, hx.slice(256, 126), ACT_RELU);
+    if (debug_ && it == r.iters - 1) tap_copy(cx, "raft.motion_last", mot);   // 126 motion features + the 2 flow channels
     // SepConvGRU raft/update.py:35-73 (horizontal 1x5 then vertical 5x1)
     for (const char* sfx : {"1", "2"}) {
       if (hoist) {
@@ -1038,6 +1042,7 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
       // the mask head and the convex upsampling (raft/raft.py:155-163): every iteration for flow_predictions, else the last one only
       N.conv(u + ".mask.0", hcur, fh, ACT_RELU);
       N.conv(u + ".mask.2", fh, mask);
+      if (last) tap("raft.mask", mask);   // (0.25 is folded into mask.2's weights)
       coords_minus_grid(cx, coords1, flow, TV());
       const TV& up = last ? r.flow_up : up_it;
       if (last) tap("raft.lowres_flow_final", flow);
@@ -1758,7 +1763,8 @@ size_t Engine::plan_raft(int n_frames, int h, int w, int n_pairs, int outputs) {
   for (int s = 0; s < n_pairs; ++s) { src[s] = s % n_frames; tgt[s] = (s + 1) % n_frames; }
   RaftOutputs o; o.flow_up = o.flow_low = o.feat4 = o.feat8 = o.fmap = kFake;
   if (outputs & GIMMVFI_RAFT_OUT_ITERS) o.flow_iters = kFake;
-  return dry_run([&](Ctx& cx) { run_raft_pairs(cx, kFake, n_frames, h, w, src, tgt, 1, nullptr, o, true); });
+  // debug: 5 iterations, so that the snapshots of iterations 0 and 4 and those of the last iteration are all planned
+  return dry_run([&](Ctx& cx) { run_raft_pairs(cx, kFake, n_frames, h, w, src, tgt, debug_ ? 5 : 1, nullptr, o, true); });
 }
 
 void Engine::forward_raft(const float* frames, int n_frames, int h, int w, const int32_t* pairs, int n_pairs, int iters, const float* flow_init,

@@ -174,16 +174,21 @@ def corr_lookup(pyr: List[Tensor], coords: Tensor, r=4) -> Tensor:
     return torch.cat(out, dim=-1).permute(0, 3, 1, 2).contiguous().to(pyr[0].dtype)
 
 
-def raft_update_block(sd: SD, p: str, net: Tensor, inp: Tensor, corr: Tensor, flow: Tensor):
-    """raft/update.py:131-154 (BasicMotionEncoder :94-112, SepConvGRU :35-73,
-    FlowHead :6-14, mask head :139-143)."""
+def raft_motion_encoder(sd: SD, p: str, corr: Tensor, flow: Tensor) -> Tensor:
+    """raft/update.py:94-112 (BasicMotionEncoder) → 126 motion features | the 2 flow channels."""
     e = p + ".encoder"
     cor = F.relu(_conv(sd, e + ".convc1", corr))
     cor = F.relu(_conv(sd, e + ".convc2", cor, padding=1))
     flo = F.relu(_conv(sd, e + ".convf1", flow, padding=3))
     flo = F.relu(_conv(sd, e + ".convf2", flo, padding=1))
     out = F.relu(_conv(sd, e + ".conv", torch.cat([cor, flo], 1), padding=1))
-    motion = torch.cat([out, flow], 1)
+    return torch.cat([out, flow], 1)
+
+
+def raft_update_block(sd: SD, p: str, net: Tensor, inp: Tensor, corr: Tensor, flow: Tensor):
+    """raft/update.py:131-154 (BasicMotionEncoder :94-112, SepConvGRU :35-73,
+    FlowHead :6-14, mask head :139-143)."""
+    motion = raft_motion_encoder(sd, p, corr, flow)
     x = torch.cat([inp, motion], 1)
     g = p + ".gru"
     h = net

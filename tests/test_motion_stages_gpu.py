@@ -22,10 +22,10 @@ import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import gimmvfi_r_oracle as O
 from gimmvfi_b200.synth import synth_batch
+from corr_ref import corr_direct64
 from splat_ref import splat_w_bound, splat_w_float64
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim"))
@@ -204,41 +204,6 @@ def splat64(lat, flow, metric):
     bound = torch.where(cnt == 0, torch.zeros_like(bound), bound)   # no source reaches the pixel: both give exactly 0
     shape = lambda t: t.view(N, H, W, -1).permute(0, 3, 1, 2)
     return shape(out), shape(bound)
-
-
-def corr_direct64(fsrc, ftgt, coords, r=4, chunk=2048):
-    """BidirCorrBlock's lookup (raft/corr.py:23-93 == oracle.BidirCorr + corr_lookup) without the volume: at level l the 2r+2 x 2r+2
-    integer neighbours of each window on the 2^l-average-pooled target features (pooling the volume's target dims is pooling the
-    features: the dot product is linear), zero outside the frame, then the bilinear weights.  fsrc / ftgt (N, C, h, w), coords (N, 2, h, w)
-    (x, y) at level 0 -> (N, 4 (2r+1)^2, h, w); channel i (2r+1) + j of a level samples (Δx, Δy) = (i - r, j - r)."""
-    N, C, h, w = fsrc.shape
-    k = 2 * r + 1
-    pyr = [ftgt]
-    for _ in range(3):
-        pyr.append(F.avg_pool2d(pyr[-1], 2, stride=2))
-    src = fsrc.permute(0, 2, 3, 1).reshape(N, h * w, C)
-    cen0 = coords.permute(0, 2, 3, 1).reshape(N, h * w, 2)
-    offs = torch.arange(-r, r + 2, device=fsrc.device)
-    out = torch.empty(N, h * w, 4 * k * k, device=fsrc.device, dtype=fsrc.dtype)
-    for l, ft in enumerate(pyr):
-        hl, wl = ft.shape[-2:]
-        tgt = ft.permute(0, 2, 3, 1).reshape(N, hl * wl, C)
-        cen = cen0 / 2 ** l
-        for n in range(N):
-            for p0 in range(0, h * w, chunk):
-                c = cen[n, p0:p0 + chunk]
-                x0, y0 = torch.floor(c[:, 0]), torch.floor(c[:, 1])
-                fx, fy = (c[:, 0] - x0).view(-1, 1, 1), (c[:, 1] - y0).view(-1, 1, 1)
-                xs = x0.long().view(-1, 1) + offs                                  # (P, 2r+2)
-                ys = y0.long().view(-1, 1) + offs
-                valid = ((ys >= 0) & (ys < hl)).unsqueeze(2) & ((xs >= 0) & (xs < wl)).unsqueeze(1)   # (P, y, x)
-                idx = ys.clamp(0, hl - 1).unsqueeze(2) * wl + xs.clamp(0, wl - 1).unsqueeze(1)
-                g = tgt[n][idx]                                                     # (P, 2r+2, 2r+2, C)
-                d = torch.einsum("pabc,pc->pab", g, src[n, p0:p0 + chunk]) / math.sqrt(C) * valid
-                s = ((1 - fx) * (1 - fy) * d[:, :k, :k] + fx * (1 - fy) * d[:, :k, 1:] + (1 - fx) * fy * d[:, 1:, :k]
-                     + fx * fy * d[:, 1:, 1:])                                      # (P, Δy, Δx)
-                out[n, p0:p0 + chunk, l * k * k:(l + 1) * k * k] = s.transpose(1, 2).reshape(-1, k * k)
-    return out.view(N, h, w, -1).permute(0, 3, 1, 2)
 
 
 def lookup_coords64(fl4, t):
