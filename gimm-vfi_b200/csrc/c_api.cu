@@ -440,6 +440,13 @@ int gimmvfi_op_corr_volume_tc(const gimmvfi_view* fa, const gimmvfi_view* fb, fl
     TV a = to_tv(fa); TV b = to_tv(fb);
     if (a.n != 1 || b.n != 1 || a.c % 32 || a.ld != a.c || b.ld != b.c) throw std::runtime_error("corr_volume_tc: one dense sample with C % 32 == 0");
     const int64_t N = (int64_t)a.h * a.w;
+    if ((int64_t)b.h * b.w != N) throw std::runtime_error("corr_volume_tc: fa and fb must have the same number of pixels");
+    if (split && corr_volume_tc_wants_f16_planes() && a.c % 64 == 0) {   // half planes of fa, then of fb: 2 N C floats of scratch
+      uint16_t* ap = reinterpret_cast<uint16_t*>(scratch); uint16_t* bp = ap + 2 * N * a.c;
+      split_planes_f16(cx, a, ap); split_planes_f16(cx, b, bp);
+      corr_gemm_3xf16(cx, ap, N * a.c, (int)N, bp, N * a.c, (int)N, a.c, 1.0f / std::sqrt((float)a.c), vol);
+      return 0;
+    }
     float* planes = scratch; float* zeros = scratch + 2 * N * a.c;
     dev_memset(zeros, 0, (size_t)(((N + 255) / 256) * 256 + 512) * sizeof(float), cx.stream);
     if (split && corr_volume_tc_wants_f16_planes()) split_planes_f16(cx, b, planes);

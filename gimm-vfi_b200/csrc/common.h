@@ -363,6 +363,10 @@ bool conv2d_tc_supported(const TV& in0, const TV& in1, const ConvW& w, const Con
 void conv2d_tc(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out, bool split);
 void corr_volume_tc(Ctx& cx, const TV& fa, const float* fb_planes, const float* zero_bias, float* vol, float scale, bool split, int n_targets = 0);
 bool corr_volume_tc_wants_f16_planes();   // split mode: true -> fb_planes must come from split_planes_f16 (3xF16 form), else split_planes
+// corr_gemm.cu (sm_90a): vol[i][j] = scale * <A[i,:], B[j,:]> in the 3xF16 form, row pitch NT; A / B = half planes [2][rows][K] from
+// split_planes_f16 (a_plane / b_plane: elements from the hi to the lo plane), K % 64 == 0
+void corr_gemm_3xf16(Ctx& cx, const void* a_planes, int64_t a_plane, int M, const void* b_planes, int64_t b_plane, int NT, int K, float scale,
+                     float* vol);
 // conv_halo.cu (sm_90a): 3x3 / 1x1 stride-1 convolutions of K-poor layers (cin <= 32 fp32 / 64 half, cout <= 64) with the activation
 // tile + halo loaded once (three x-shifted copies) and every tap an MMA on a 1024-byte aligned view of it, weights resident
 bool conv2d_halo_supported(const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out);

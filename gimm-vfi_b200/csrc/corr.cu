@@ -125,6 +125,12 @@ void split_planes_f16(Ctx& cx, const TV& src, void* planes) {
   int64_t n = src.pixels() * src.c;
   parallel_for(cx, n, SplitPlanesF16K{src, static_cast<uint16_t*>(planes), n}, "split_planes");
 }
+#ifdef GV_HOSTSIM
+// (the host simulation takes the TF32 planes: corr_volume_tc_wants_f16_planes() is false there)
+void corr_gemm_3xf16(Ctx&, const void*, int64_t, int, const void*, int64_t, int, int, float, float*) {
+  throw std::runtime_error("corr_gemm_3xf16 is a tensor-core kernel; not available in the host simulation");
+}
+#endif
 
 // 2x2 average of an NHWC feature map (floor semantics): the targets of pyramid level l are the level-(l-1) features pooled
 struct PoolFeatK {

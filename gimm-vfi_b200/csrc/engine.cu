@@ -757,7 +757,7 @@ static std::vector<std::pair<int, int>> pair_runs(const std::vector<int>& src, c
 
 // One volume per pair on the batch axis: sample s holds <F[src[s]], F[tgt[s]]> (GIMM-VFI-R's second direction is the transposed
 // volume, raft/corr.py:32).  Level l is (P*N) x (h_l*w_l).
-// tc: 0 = fp32 CUDA-core GEMM, 1 = wgmma plain TF32, 2 = wgmma 3xTF32 (promoted accumulation)
+// tc: 0 = fp32 CUDA-core GEMM, 1 = wgmma plain TF32, 2 = wgmma 3xF16 (corr_gemm_3xf16) or 3xTF32 (promoted accumulation)
 static Pyramid build_pyramid(Ctx& cx, const TV& F /*frames,h,w,256*/, const std::vector<int>& src, const std::vector<int>& tgt, int tensor_cores) {
   Arena& A = cx.arena;
   const int S = (int)src.size();
@@ -772,13 +772,32 @@ static Pyramid build_pyramid(Ctx& cx, const TV& F /*frames,h,w,256*/, const std:
     // (1088x1920) is never re-read (the pooling pass over it took as long as the GEMM that wrote it).
     const bool split = tensor_cores >= 2;
     const size_t mk = A.mark();
+    TV Fl[4]; Fl[0] = F;
+    for (int l = 1; l < 4; ++l) { Fl[l] = A.tensor(F.n, P.h[l], P.w[l], F.c); avgpool2_features(cx, Fl[l - 1], Fl[l]); }
+    if (split && corr_volume_tc_wants_f16_planes() && F.c % 64 == 0) {
+      // 3xF16 on pre-split operands: every frame's features are split once per level; a frame's level-0 planes are the sources of
+      // its own pairs and the targets of the reverse direction
+      uint16_t* pl[4]; int64_t plane[4];
+      for (int l = 0; l < 4; ++l) {
+        plane[l] = (int64_t)F.n * P.h[l] * P.w[l] * F.c;
+        pl[l] = reinterpret_cast<uint16_t*>(A.alloc_f((size_t)plane[l]));   // 2 half planes
+        if (P.h[l] * P.w[l] > 0) split_planes_f16(cx, Fl[l], pl[l]);
+      }
+      for (int s = 0; s < S; ++s)
+        for (int l = 0; l < 4; ++l) {
+          const int nt = P.h[l] * P.w[l];
+          if (nt <= 0 || cx.dry) continue;
+          corr_gemm_3xf16(cx, pl[0] + (int64_t)src[s] * P.N * F.c, plane[0], (int)P.N, pl[l] + (int64_t)tgt[s] * nt * F.c, plane[l], nt, F.c, scale,
+                          P.lvl[l] + (int64_t)s * P.N * nt);
+        }
+      A.release(mk);
+      return P;
+    }
     const int64_t plane = (int64_t)P.N * F.c;
     float* planes = A.alloc_f((size_t)2 * plane);
     const int64_t nz = ((P.N + 255) / 256) * 256 + 512;
     float* zeros = A.alloc_f((size_t)nz);
     if (!cx.dry) dev_memset(zeros, 0, (size_t)nz * sizeof(float), cx.stream);
-    TV Fl[4]; Fl[0] = F;
-    for (int l = 1; l < 4; ++l) { Fl[l] = A.tensor(F.n, P.h[l], P.w[l], F.c); avgpool2_features(cx, Fl[l - 1], Fl[l]); }
     for (int s = 0; s < S; ++s) {
       const int other = tgt[s];
       for (int l = 0; l < 4; ++l) {

@@ -289,7 +289,15 @@ struct FF {
   void cost_volume(const TV& F, const std::vector<int>& src, const std::vector<int>& tgt, float* vol) {
     const int64_t Npx = (int64_t)F.h * F.w;
     const int S = (int)src.size();
-    if (cx.tc && F.c % 64 == 0 && F.ld == F.c) {
+    if (cx.tc && F.c % 64 == 0 && F.ld == F.c && corr_volume_tc_wants_f16_planes()) {   // every frame split once
+      const size_t mk = A.mark();
+      const int64_t plane = F.n * Npx * F.c;
+      uint16_t* pl = reinterpret_cast<uint16_t*>(A.alloc_f((size_t)plane));
+      split_planes_f16(cx, F, pl);
+      for (int s = 0; s < S; ++s)
+        if (!cx.dry) corr_gemm_3xf16(cx, pl + src[s] * Npx * F.c, plane, (int)Npx, pl + tgt[s] * Npx * F.c, plane, (int)Npx, F.c, 1.0f, vol + (int64_t)s * Npx * Npx);
+      A.release(mk);
+    } else if (cx.tc && F.c % 64 == 0 && F.ld == F.c) {
       const size_t mk = A.mark();
       float* planes = A.alloc_f((size_t)2 * Npx * F.c);
       const int64_t nz = ((Npx + 255) / 256) * 256 + 512;
@@ -465,7 +473,14 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     conv2d(cx, hx.slice(128, 128), TV(), wa, ConvGeom(), ConvEpi(), q);
     conv2d(cx, hx.slice(128, 128), TV(), wb, ConvGeom(), ConvEpi(), k);
     const float scale = 1.0f / std::sqrt(128.f);
-    if (cx.tc) {
+    if (cx.tc && corr_volume_tc_wants_f16_planes()) {
+      const int64_t plane = (int64_t)S * Npx * 128;
+      uint16_t* qp = reinterpret_cast<uint16_t*>(A.alloc_f((size_t)plane));
+      uint16_t* kp = reinterpret_cast<uint16_t*>(A.alloc_f((size_t)plane));
+      split_planes_f16(cx, q, qp); split_planes_f16(cx, k, kp);
+      for (int s = 0; s < S; ++s)
+        if (!cx.dry) corr_gemm_3xf16(cx, qp + s * Npx * 128, plane, (int)Npx, kp + s * Npx * 128, plane, (int)Npx, 128, scale, att + (int64_t)s * Npx * Npx);
+    } else if (cx.tc) {
       float* planes = A.alloc_f((size_t)2 * Npx * 128);
       const int64_t nz = ((Npx + 255) / 256) * 256 + 512;
       float* zb = A.alloc_f((size_t)nz);
