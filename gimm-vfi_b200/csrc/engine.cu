@@ -1825,7 +1825,8 @@ size_t Engine::plan_flowformer(int n_frames, int h, int w, int n_pairs) {
   std::vector<int> src(n_pairs), tgt(n_pairs);
   for (int s = 0; s < n_pairs; ++s) { src[s] = s % n_frames; tgt[s] = (s + 1) % n_frames; }
   FlowFormerOutputs o; o.flow_up = o.flow_low = kFake;
-  return dry_run([&](Ctx& cx) { run_flowformer_pairs(cx, kFake, n_frames, h, w, src, tgt, 1, 1, true, nullptr, o); });
+  // debug: 2 iterations, so that the snapshots of iteration 0 and those of the last iteration are planned in the order a forward takes them
+  return dry_run([&](Ctx& cx) { run_flowformer_pairs(cx, kFake, n_frames, h, w, src, tgt, 1, debug_ ? 2 : 1, true, nullptr, o); });
 }
 
 void Engine::forward_flowformer(const float* frames, int n_frames, int h, int w, const int32_t* pairs, int n_pairs, int pairs_per_call, int iters,

@@ -361,6 +361,7 @@ struct FF {
     lin_res(il + ".proj", att, TV(), x2, x);
     mlp(il + ".norm2", 1e-5f, il + ".ffn.0", il + ".ffn.3", x, sc);       // sc = short_cut (encoder.py:470)
     copy_channels(cx, sc, x);
+    E.tap_pub("ff.latent_in", sc);                                        // (kept in debug mode: mk0 is not released then)
     for (int i = 0; i < 3; ++i) {
       const std::string e = p + ".encoder_layers." + std::to_string(i);
       {   // SelfAttentionLayer over the 8 tokens of every cost map (encoder.py:248-266)
@@ -439,7 +440,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     f.lin(me + ".channel_convertor", t8, fproj);
     A.release(mk);
   }
-  tap("ff.feat8", feat8); tap("ff.fproj", fproj);
+  tap("ff.feat4", feat4); tap("ff.feat8", feat8); tap("ff.fproj", fproj);
   if (encoded) encoded(feat4, feat8, fproj);
   TV ctx8 = feat8;   // the context of every pair (decoder proj, GMA, the vertical blocks' concat_pe), in pair order
   if (!in_order) {
@@ -449,6 +450,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
   // ---- memory encoder
   float* vol = A.alloc_f((size_t)S * Npx * Npx);
   f.cost_volume(fproj, src, tgt, vol);
+  tap("ff.cost_volume", make_tv(vol, S, h, w, (int)Npx));   // [pair][source pixel][target pixel]
   TV latent = A.tensor(S * 8, h, w, 128);
   f.cost_perceiver(me + ".cost_perceiver_encoder", S, per_call, vol, h, w, ctx8, latent);
   tap("ff.cost_memory", latent);
@@ -462,6 +464,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     ConvEpi e1; e1.act1 = ACT_TANH; conv2d(cx, ctx8, TV(), wa, ConvGeom(), e1, hcur);
     ConvEpi e2; e2.act1 = ACT_RELU; conv2d(cx, ctx8, TV(), wb, ConvGeom(), e2, hx.slice(128, 128));
   }
+  tap_copy(cx, "ff.cnet", hx.slice(0, 256));   // tanh(net) | relu(inp) (the GRU overwrites net in place)
   // GMA attention (gma.py:56-76), once per pair: softmax(q k^T / sqrt(128)) stored * att_mul (a power of two)
   float att_mul = 1.f;
   while (att_mul < (float)Npx && att_mul < 32768.f) att_mul *= 2.f;   // (<= 2^15: a one-hot row stays below the largest half)
@@ -498,6 +501,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     row_softmax(cx, att, (int64_t)S * Npx, Npx, att_mul);
     A.release(mk);
   }
+  tap("ff.gma_attn", make_tv(att, S, h, w, (int)Npx));   // softmax rows * att_mul
   const bool agg_tc = cx.tc && Npx % 64 == 0;
   float* vt_planes = nullptr; float* vT = nullptr;
   if (agg_tc) {
@@ -531,6 +535,8 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
   for (int l = 0; l < 4; ++l) { pyr.lvl[l] = vol; pyr.h[l] = h; pyr.w[l] = w; }
   pyr.rows_per_sample = Npx; pyr.nl = 1;
   for (int it = 0; it < iters; ++it) {
+    const bool last = it == iters - 1;
+    if (last) { tap_copy(cx, "ff.coords_last", coords1); tap_copy(cx, "ff.net_last", hcur); }
     // encode_flow_token: 9x9 window of each pixel's own cost map around its current target (decoder.py:233-252)
     corr_lookup(cx, pyr, coords1, cfw);
     f.lin(md + ".flow_token_encoder.0", cfw, ft1, ACT_GELU);
@@ -550,6 +556,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     f.mlp(ca + ".norm2", 1e-5f, ca + ".ffn.0", ca + ".ffn.3", xg, cgl);
     coords_minus_grid(cx, coords1, flow, hx.slice(382, 2));
     if (it == 0) tap_copy(cx, "ff.dec_corr_0", corr);
+    if (last) tap_copy(cx, "ff.corr_last", corr);
     // BasicMotionEncoder (gru.py:75-97)
     N.conv(u + ".encoder.convc1", corr, cor1, ACT_RELU);
     N.conv(u + ".encoder.convc2", cor1, corflo.slice(0, 192), ACT_RELU);
@@ -571,6 +578,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
       }
     }
     axpy_dev(cx, mf, agg, N.V(u + ".aggregator.gamma"), mg);
+    if (last) { tap_copy(cx, "ff.motion_last", mf); tap_copy(cx, "ff.mg_last", mg); }   // (126 motion features + the 2 flow channels | mg)
     // SepConvGRU (gru.py:35-73) over [h | inp | mf | mg]
     for (const char* sfx : {"1", "2"}) {
       if (hoist) {
@@ -596,9 +604,10 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
     if (it == 0) tap_copy(cx, "ff.dec_net_0", hcur);
     N.conv(u + ".flow_head.conv1", hcur, fh, ACT_RELU);
     { ConvEpi e; e.res = coords1; N.conv_e(u + ".flow_head.conv2", fh, TV(), coords1, e); }
-    if (it == iters - 1) {   // only the last prediction is consumed (decoder.py:321, gimmvfi_f.py:122-123)
+    if (last) {   // only the last prediction is consumed (decoder.py:321, gimmvfi_f.py:122-123)
       N.conv(u + ".mask.0", hcur, fh, ACT_RELU);
       N.conv(u + ".mask.2", fh, mask);
+      tap("ff.net_final", hcur); tap("ff.mask", mask);   // (0.25 is folded into mask.2's weights)
       coords_minus_grid(cx, coords1, flow, TV());
       tap("ff.lowres_flow", flow);
       if (flow_low.p) copy_channels(cx, flow, flow_low);

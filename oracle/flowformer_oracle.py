@@ -26,15 +26,17 @@ def _ln(sd, k, x, eps):
     return F.layer_norm(x, (x.shape[-1],), sd[k + ".weight"], sd[k + ".bias"], eps)
 
 
-def coords_grid(b, h, w):
-    """flowformer/core/utils/utils.py coords_grid: channel 0 = x, channel 1 = y."""
-    ys, xs = torch.meshgrid(torch.arange(h), torch.arange(w), indexing="ij")
-    return torch.stack([xs, ys], 0).float()[None].repeat(b, 1, 1, 1)
+def coords_grid(b, h, w, like=None):
+    """flowformer/core/utils/utils.py coords_grid: channel 0 = x, channel 1 = y.  With `like`: on its device, in its dtype (else fp32 on
+    the CPU)."""
+    dev = like.device if like is not None else None
+    ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
+    return torch.stack([xs, ys], 0).to(like.dtype if like is not None else torch.float32)[None].repeat(b, 1, 1, 1)
 
 
 def linear_pos_embedding_sine(x, dim=128):
     """LCF/attention.py:170-182 (the constant is 3.14, not pi)."""
-    fb = torch.linspace(0, dim // 4 - 1, dim // 4)
+    fb = torch.linspace(0, dim // 4 - 1, dim // 4, dtype=x.dtype, device=x.device)
     k = 1 / 200
     return torch.cat([torch.sin(3.14 * x[..., -2:-1] * fb * k), torch.cos(3.14 * x[..., -2:-1] * fb * k),
                       torch.sin(3.14 * x[..., -1:] * fb * k), torch.cos(3.14 * x[..., -1:] * fb * k)], -1)
@@ -145,7 +147,7 @@ def vertical_local(sd, b, x, size, context, heads=8, ws=7):
     yqk = yqk.reshape(B, _h, ws, _w, ws, Cqk).transpose(2, 3)
     hd = C // heads
     v = _lin(sd, a + ".v", y).reshape(B, _h * _w, ws * ws, heads, hd).transpose(2, 3)
-    pe = linear_pos_embedding_sine(coords_grid(B, ws, ws).view(B, 2, -1).permute(0, 2, 1), dim=Cqk).view(B, ws, ws, Cqk)
+    pe = linear_pos_embedding_sine(coords_grid(B, ws, ws, y).view(B, 2, -1).permute(0, 2, 1), dim=Cqk).view(B, ws, ws, Cqk)
     yqk = yqk + pe[:, None, None]
     q = _lin(sd, a + ".q", yqk).reshape(B, _h * _w, ws * ws, heads, hd).transpose(2, 3)
     k = _lin(sd, a + ".k", yqk).reshape(B, _h * _w, ws * ws, heads, hd).transpose(2, 3)
@@ -173,13 +175,13 @@ def vertical_global(sd, b, x, size, context, heads=8, sr=4):
     hd = C // heads
     y = y.view(B, -1, C)
     yqk = yqk.view(B, -1, Cqk)
-    pe = linear_pos_embedding_sine(coords_grid(B, Hp, Wp).view(B, 2, -1).permute(0, 2, 1), dim=Cqk)
+    pe = linear_pos_embedding_sine(coords_grid(B, Hp, Wp, y).view(B, 2, -1).permute(0, 2, 1), dim=Cqk)
     q = _lin(sd, a + ".q", yqk + pe).reshape(B, Hp * Wp, heads, hd).permute(0, 2, 1, 3)
     ys = F.conv2d(y.permute(0, 2, 1).reshape(B, C, Hp, Wp), sd[a + ".sr_value.weight"], sd[a + ".sr_value.bias"], stride=sr)
     yk = F.conv2d(yqk.permute(0, 2, 1).reshape(B, Cqk, Hp, Wp), sd[a + ".sr_key.weight"], sd[a + ".sr_key.bias"], stride=sr)
     ys = _ln(sd, a + ".norm", ys.reshape(B, C, -1).permute(0, 2, 1), 1e-5)
     yk = _ln(sd, a + ".norm", yk.reshape(B, C, -1).permute(0, 2, 1), 1e-5)
-    pe2 = linear_pos_embedding_sine(coords_grid(B, Hp // sr, Wp // sr).view(B, 2, -1).permute(0, 2, 1) * sr, dim=C)
+    pe2 = linear_pos_embedding_sine(coords_grid(B, Hp // sr, Wp // sr, y).view(B, 2, -1).permute(0, 2, 1) * sr, dim=C)
     k = _lin(sd, a + ".k", yk + pe2).reshape(B, -1, heads, hd).permute(0, 2, 1, 3)
     v = _lin(sd, a + ".v", ys).reshape(B, -1, heads, hd).permute(0, 2, 1, 3)
     att = torch.softmax(q @ k.transpose(-2, -1) * hd ** -0.5, -1)
@@ -196,7 +198,7 @@ def cost_patch_embed(sd, p, cost_maps, patch=8, dim=64):
     x = F.relu(F.conv2d(x, sd[p + ".proj.2.weight"], sd[p + ".proj.2.bias"], stride=2, padding=2))
     x = F.conv2d(x, sd[p + ".proj.4.weight"], sd[p + ".proj.4.bias"], stride=2, padding=2)
     size = x.shape[2:]
-    pc = (coords_grid(B, *size) * patch + patch / 2).view(B, 2, -1).permute(0, 2, 1)
+    pc = (coords_grid(B, *size, x) * patch + patch / 2).view(B, 2, -1).permute(0, 2, 1)
     pe = linear_pos_embedding_sine(pc, dim=dim).permute(0, 2, 1).view(B, -1, *size)
     x = torch.cat([x, pe], 1)
     x = F.conv2d(F.relu(F.conv2d(x, sd[p + ".ffn_with_coord.0.weight"], sd[p + ".ffn_with_coord.0.bias"])),
@@ -208,6 +210,35 @@ def _ffn(sd, p, x):
     return _lin(sd, p + ".ffn.3", F.gelu(_lin(sd, p + ".ffn.0", x)))
 
 
+def cost_input_layer(sd, p, tokens):
+    """input_layer: CrossAttentionLayer, LCF/encoder.py:275-343 (8 heads; the 8 latent queries are shared by every cost map).
+    tokens (maps, n, 128) from cost_patch_embed -> (maps, 8, 128)"""
+    il = p + ".input_layer"
+    lat = sd[p + ".latent_tokens"]
+    qn = _ln(sd, il + ".norm1", lat, 1e-5)
+    o = mha(_lin(sd, il + ".q", qn), _lin(sd, il + ".k", tokens), _lin(sd, il + ".v", tokens), 8)
+    x = lat + _lin(sd, il + ".proj", o)
+    return x + _ffn(sd, il, _ln(sd, il + ".norm2", x, 1e-5))
+
+
+def cost_perceiver_layer(sd, p, i, x, size, context):
+    """Layer i of CostPerceiverEncoder's loop, LCF/encoder.py:477-492: the SelfAttentionLayer over the 8 latent tokens of every cost map
+    (encoder.py:209-272), then the vertical Twins blocks over each token's map.  x (B*H1*W1, 8, 128) -> the same; context (B, 256, H1, W1)
+    of the B pairs of one reference call (each block repeats it over the B*8 token maps)."""
+    H1, W1 = size
+    B = x.shape[0] // (H1 * W1)
+    e = "%s.encoder_layers.%d" % (p, i)
+    y = _ln(sd, e + ".norm1", x, 1e-5)
+    o = mha(_lin(sd, e + ".q", y), _lin(sd, e + ".k", y), _lin(sd, e + ".v", y), 8)
+    x = x + _lin(sd, e + ".proj", o)
+    x = x + _ffn(sd, e, _ln(sd, e + ".norm2", x, 1e-5))
+    x = x.view(B, H1 * W1, 8, -1).permute(0, 2, 1, 3).reshape(B * 8, H1 * W1, -1)                    # LCF/encoder.py:481-491
+    v = "%s.vertical_encoder_layers.%d" % (p, i)
+    x = vertical_local(sd, v + ".local_block", x, (H1, W1), context)
+    x = vertical_global(sd, v + ".global_block", x, (H1, W1), context)
+    return x.view(B, 8, H1 * W1, -1).permute(0, 2, 1, 3).reshape(B * H1 * W1, 8, -1)
+
+
 def cost_perceiver_encoder(sd, p, cost_volume, context, taps=None):
     """CostPerceiverEncoder.forward, LCF/encoder.py:450-495.  cost_volume (B,1,H1,W1,H2,W2) -> cost memory (B*H1*W1, 8, 128)."""
     B, heads, H1, W1, H2, W2 = cost_volume.shape
@@ -215,27 +246,12 @@ def cost_perceiver_encoder(sd, p, cost_volume, context, taps=None):
     x, size = cost_patch_embed(sd, p + ".patch_embed", cost_maps)
     if taps is not None:
         taps["patch_tokens"] = x
-    # input_layer: CrossAttentionLayer, LCF/encoder.py:275-343 (8 heads; the 8 latent queries are shared by every cost map)
-    il = p + ".input_layer"
-    lat = sd[p + ".latent_tokens"]
-    qn = _ln(sd, il + ".norm1", lat, 1e-5)
-    o = mha(_lin(sd, il + ".q", qn), _lin(sd, il + ".k", x), _lin(sd, il + ".v", x), 8)
-    x = lat + _lin(sd, il + ".proj", o)
-    x = x + _ffn(sd, il, _ln(sd, il + ".norm2", x, 1e-5))
+    x = cost_input_layer(sd, p, x)
     short_cut = x
     if taps is not None:
         taps["latent_in"] = x
     for i in range(3):
-        e = "%s.encoder_layers.%d" % (p, i)                                                          # SelfAttentionLayer, LCF/encoder.py:209-272
-        y = _ln(sd, e + ".norm1", x, 1e-5)
-        o = mha(_lin(sd, e + ".q", y), _lin(sd, e + ".k", y), _lin(sd, e + ".v", y), 8)
-        x = x + _lin(sd, e + ".proj", o)
-        x = x + _ffn(sd, e, _ln(sd, e + ".norm2", x, 1e-5))
-        x = x.view(B, H1 * W1, 8, -1).permute(0, 2, 1, 3).reshape(B * 8, H1 * W1, -1)                # LCF/encoder.py:481-491
-        v = "%s.vertical_encoder_layers.%d" % (p, i)
-        x = vertical_local(sd, v + ".local_block", x, (H1, W1), context)
-        x = vertical_global(sd, v + ".global_block", x, (H1, W1), context)
-        x = x.view(B, 8, H1 * W1, -1).permute(0, 2, 1, 3).reshape(B * H1 * W1, 8, -1)
+        x = cost_perceiver_layer(sd, p, i, x, (H1, W1), context)
         if taps is not None:
             taps["latent_%d" % i] = x
     return x + short_cut, cost_maps, size
@@ -261,7 +277,7 @@ def encode_flow_token(cost_maps, coords):
     """LCF/decoder.py:233-252: 9x9 bilinear window around coords in each pixel's own cost map (x + dy[i], y + dx[j]: the transposed window)."""
     coords = coords.permute(0, 2, 3, 1)
     b, h1, w1, _ = coords.shape
-    d = torch.linspace(-4, 4, 9)
+    d = torch.linspace(-4, 4, 9, dtype=coords.dtype, device=coords.device)
     delta = torch.stack(torch.meshgrid(d, d, indexing="ij"), -1).view(1, 9, 9, 2)
     corr = bilinear_sampler(cost_maps, coords.reshape(b * h1 * w1, 1, 1, 2) + delta)
     return corr.view(b, h1, w1, -1).permute(0, 3, 1, 2)
@@ -271,16 +287,23 @@ def _conv(sd, k, x, pad=0):
     return F.conv2d(x, sd[k + ".weight"], sd.get(k + ".bias"), padding=pad)
 
 
-def gma_update_block(sd, u, net, inp, corr, flow, attention, last):
-    """GMAUpdateBlock.forward, LCF/gru.py:130-160 (+ BasicMotionEncoder :75-97, Aggregate gma.py:84-115, SepConvGRU :35-73)."""
+def motion_encoder(sd, u, corr, flow):
+    """BasicMotionEncoder, LCF/gru.py:75-97: corr (B,145,h,w), flow (B,2,h,w) -> motion features | flow (B,128,h,w)"""
     e = u + ".encoder"
     cor = F.relu(_conv(sd, e + ".convc2", F.relu(_conv(sd, e + ".convc1", corr)), 1))
     flo = F.relu(_conv(sd, e + ".convf2", F.relu(_conv(sd, e + ".convf1", flow, 3)), 1))
-    mf = torch.cat([F.relu(_conv(sd, e + ".conv", torch.cat([cor, flo], 1), 1)), flow], 1)
+    return torch.cat([F.relu(_conv(sd, e + ".conv", torch.cat([cor, flo], 1), 1)), flow], 1)
+
+
+def aggregate(sd, u, mf, attention):
+    """Aggregate, gma.py:84-115: mf + gamma * (attention @ to_v(mf)); attention (B,1,N,N)"""
     b, c, h, w = mf.shape
     v = _conv(sd, u + ".aggregator.to_v", mf).view(b, 1, c, h * w).transpose(2, 3)
-    mg = mf + sd[u + ".aggregator.gamma"] * (attention @ v).transpose(2, 3).reshape(b, c, h, w)
-    x = torch.cat([inp, mf, mg], 1)
+    return mf + sd[u + ".aggregator.gamma"] * (attention @ v).transpose(2, 3).reshape(b, c, h, w)
+
+
+def sep_conv_gru(sd, u, net, x):
+    """SepConvGRU, LCF/gru.py:35-73: net (B,128,h,w), x = [inp | mf | mg] (B,384,h,w)"""
     g = u + ".gru"
     for s, pad in (("1", (0, 2)), ("2", (2, 0))):
         hx = torch.cat([net, x], 1)
@@ -288,9 +311,24 @@ def gma_update_block(sd, u, net, inp, corr, flow, attention, last):
         r = torch.sigmoid(_conv(sd, g + ".convr" + s, hx, pad))
         q = torch.tanh(_conv(sd, g + ".convq" + s, torch.cat([r * net, x], 1), pad))
         net = (1 - z) * net + z * q
-    dflow = _conv(sd, u + ".flow_head.conv2", F.relu(_conv(sd, u + ".flow_head.conv1", net, 1)), 1)
-    mask = 0.25 * _conv(sd, u + ".mask.2", F.relu(_conv(sd, u + ".mask.0", net, 1))) if last else None
-    return net, mask, dflow
+    return net
+
+
+def flow_head(sd, u, net):
+    return _conv(sd, u + ".flow_head.conv2", F.relu(_conv(sd, u + ".flow_head.conv1", net, 1)), 1)
+
+
+def mask_head(sd, u, net):
+    """0.25 * mask(net), LCF/gru.py:158"""
+    return 0.25 * _conv(sd, u + ".mask.2", F.relu(_conv(sd, u + ".mask.0", net, 1)))
+
+
+def gma_update_block(sd, u, net, inp, corr, flow, attention, last):
+    """GMAUpdateBlock.forward, LCF/gru.py:130-160 (+ BasicMotionEncoder :75-97, Aggregate gma.py:84-115, SepConvGRU :35-73)."""
+    mf = motion_encoder(sd, u, corr, flow)
+    mg = aggregate(sd, u, mf, attention)
+    net = sep_conv_gru(sd, u, net, torch.cat([inp, mf, mg], 1))
+    return net, (mask_head(sd, u, net) if last else None), flow_head(sd, u, net)
 
 
 def upsample_flow(flow, mask):
@@ -301,37 +339,54 @@ def upsample_flow(flow, mask):
     return torch.sum(mask * up, 2).permute(0, 1, 4, 2, 5, 3).reshape(N, 2, 8 * H, 8 * W)
 
 
+def gma_attention(sd, inp):
+    """Attention, gma.py:56-76 (its positional term is disabled there): softmax(q k^T / sqrt(128)) of to_qk(inp) -> (B,1,N,N)"""
+    qk = _conv(sd, P + "memory_decoder.att.to_qk", inp)
+    q, k = qk[:, :128].flatten(2).transpose(1, 2) * 128 ** -0.5, qk[:, 128:].flatten(2).transpose(1, 2)
+    return torch.softmax(q @ k.transpose(1, 2), -1)[:, None]
+
+
+def cost_global(sd, cost_forward, coords1, key, value):
+    """flow_token_encoder + the decoder's CrossAttentionLayer (LCF/decoder.py:81-117, :295-305) for one query per pixel against its 8
+    memory tokens: cost_forward (B,81,h,w), key / value (B*h*w, 8, 64) -> cost_global (B,64,h,w)"""
+    p = P + "memory_decoder"
+    ca = p + ".decoder_layer.cross_attend"
+    B, _, H1, W1 = cost_forward.shape
+    query = _conv(sd, p + ".flow_token_encoder.2", F.gelu(_conv(sd, p + ".flow_token_encoder.0", cost_forward)))
+    query = query.permute(0, 2, 3, 1).contiguous().view(B * H1 * W1, 1, 64)
+    qc = coords1.reshape(B, 2, -1).permute(0, 2, 1).reshape(B * H1 * W1, 1, 2)
+    pe = linear_pos_embedding_sine(qc, dim=64)
+    y = _ln(sd, ca + ".norm1", query, 1e-5)
+    o = mha(_lin(sd, ca + ".q", y + pe), key, value, 8)
+    x = query + _lin(sd, ca + ".proj", torch.cat([o, query], 2))
+    x = x + _ffn(sd, ca, _ln(sd, ca + ".norm2", x, 1e-5))
+    return x.view(B, H1, W1, 64).permute(0, 3, 1, 2)
+
+
+def decoder_iteration(sd, net, inp, coords0, coords1, cost_maps, key, value, attention, last):
+    """One iteration of MemoryDecoder.forward's loop, LCF/decoder.py:290-319 -> (net, the flow update, mask (last only), corr)"""
+    cost_forward = encode_flow_token(cost_maps, coords1)
+    corr = torch.cat([cost_global(sd, cost_forward, coords1, key, value), cost_forward], 1)
+    net, up_mask, dflow = gma_update_block(sd, P + "memory_decoder.update_block", net, inp, corr, coords1 - coords0, attention, last)
+    return net, dflow, up_mask, corr
+
+
 def memory_decoder(sd, cost_memory, context, cost_maps, iters=32, taps=None):
     """MemoryDecoder.forward, LCF/decoder.py:254-321 (only the last iteration's up-sampled flow is returned / needed)."""
     p = P + "memory_decoder"
     B, _, H1, W1 = context.shape
-    coords0 = coords_grid(B, H1, W1)
-    coords1 = coords_grid(B, H1, W1)
+    coords0 = coords_grid(B, H1, W1, context)
+    coords1 = coords_grid(B, H1, W1, context)
     ctx = _conv(sd, p + ".proj", context)
     net, inp = torch.tanh(ctx[:, :128]), torch.relu(ctx[:, 128:])
-    qk = _conv(sd, p + ".att.to_qk", inp)                                                           # gma.py:56-76 (positional term disabled there)
-    q, k = qk[:, :128].flatten(2).transpose(1, 2) * 128 ** -0.5, qk[:, 128:].flatten(2).transpose(1, 2)
-    attention = torch.softmax(q @ k.transpose(1, 2), -1)[:, None]
+    attention = gma_attention(sd, inp)
     ca = p + ".decoder_layer.cross_attend"
     key, value = _lin(sd, ca + ".k", cost_memory), _lin(sd, ca + ".v", cost_memory)                 # computed in iteration 0, re-used after
     flow_up = None
     for it in range(iters):
-        cost_forward = encode_flow_token(cost_maps, coords1)
-        query = _conv(sd, p + ".flow_token_encoder.2", F.gelu(_conv(sd, p + ".flow_token_encoder.0", cost_forward)))
-        query = query.permute(0, 2, 3, 1).contiguous().view(B * H1 * W1, 1, 64)
-        # CrossAttentionLayer.forward, LCF/decoder.py:81-117
-        qc = coords1.view(B, 2, -1).permute(0, 2, 1).reshape(B * H1 * W1, 1, 2)
-        pe = linear_pos_embedding_sine(qc, dim=64)
-        y = _ln(sd, ca + ".norm1", query, 1e-5)
-        o = mha(_lin(sd, ca + ".q", y + pe), key, value, 8)
-        x = query + _lin(sd, ca + ".proj", torch.cat([o, query], 2))
-        x = x + _ffn(sd, ca, _ln(sd, ca + ".norm2", x, 1e-5))
-        cost_global = x.view(B, H1, W1, 64).permute(0, 3, 1, 2)
-        corr = torch.cat([cost_global, cost_forward], 1)
-        flow = coords1 - coords0
+        net, dflow, up_mask, corr = decoder_iteration(sd, net, inp, coords0, coords1, cost_maps, key, value, attention, it == iters - 1)
         if taps is not None and it == 0:
             taps["dec_corr_0"] = corr
-        net, up_mask, dflow = gma_update_block(sd, p + ".update_block", net, inp, corr, flow, attention, it == iters - 1)
         coords1 = coords1 + dflow
         if taps is not None and it == 0:
             taps["dec_net_0"], taps["dec_dflow_0"] = net, dflow
