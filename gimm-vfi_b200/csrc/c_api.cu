@@ -310,7 +310,7 @@ int gimmvfi_op_softsplat_fused(const gimmvfi_view* lat, const gimmvfi_view* flow
   gimmvfi_engine* e = nullptr;
   GV_TRY(e, {
     Ctx cx = op_ctx(stream);
-    if (!softsplat_fused(cx, to_tv(lat), to_tv(flow), to_tv(metric), t, t_mode, flow_absmax, to_tv(out), /*force=*/true))
+    if (!softsplat_fused(cx, to_tv(lat), to_tv(flow), to_tv(metric), t, t_mode, flow_absmax, to_tv(out)))
       throw std::runtime_error("softsplat_fused: 16-channel 16-byte-aligned latent / output, 8-byte-aligned flow and a flow bound are required");
   })
 }

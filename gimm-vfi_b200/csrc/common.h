@@ -380,6 +380,9 @@ bool conv2d_tc_supported(const TV& in0, const TV& in1, const ConvW& w, const Con
 void conv2d_tc(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out, bool split);
 void corr_volume_tc(Ctx& cx, const TV& fa, const float* fb_planes, const float* zero_bias, float* vol, float scale, bool split, int n_targets = 0);
 bool corr_volume_tc_wants_f16_planes();   // split mode: true -> fb_planes must come from split_planes_f16 (3xF16 form), else split_planes
+// how long the TMA pipelines of conv_tc.cu, conv_halo.cu and corr_gemm.cu wait on an mbarrier before trapping, in units of 10 ms
+// (tc_ptx.cuh mbar_wait): GIMMVFI_TC_SPIN_LIMIT, default 400; 0 = wait forever (compute-sanitizer)
+int tc_spin_limit();
 // corr_gemm.cu (sm_90a): vol[i][j] = scale * <A[i,:], B[j,:]> in the 3xF16 form, row pitch NT; A / B = half planes [2][rows][K] from
 // split_planes_f16 (a_plane / b_plane: elements from the hi to the lo plane), K % 64 == 0
 void corr_gemm_3xf16(Ctx& cx, const void* a_planes, int64_t a_plane, int M, const void* b_planes, int64_t b_plane, int NT, int K, float scale,
@@ -464,7 +467,7 @@ void softsplat_normalize(Ctx& cx, const TV& acc, const TV& out);
 void softsplat_accumulate_mode(Ctx& cx, const TV& lat, const TV& flow, const TV& metric, const float* t_per_sample, int t_mode, const TV& acc, int mode);
 // the whole splat in one pass (target tiles in shared memory); flow_absmax[n] >= max |flow| of sample n bounds the scan region
 bool softsplat_fused(Ctx& cx, const TV& lat, const TV& flow, const TV& metric, const float* t_per_sample, int t_mode, const float* flow_absmax,
-                     const TV& out, bool force = false);
+                     const TV& out);
 // Differentiable splat of modules/softsplat.py:358-663 (softsplat_func) on 4-D strided NCHW tensors of float or double;
 // element (n,c,y,x) = p[n*s[0] + c*s[1] + y*s[2] + x*s[3]] (64-bit sizes and strides, in elements).
 template <class T> struct SV4 { T* p = nullptr; int64_t sz[4] = {0, 0, 0, 0}, st[4] = {0, 0, 0, 0}; };

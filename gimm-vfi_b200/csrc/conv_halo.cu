@@ -165,15 +165,9 @@ static void launch_halo(int grid, int smem, gvStream_t stream, const CUtensorMap
   tc::conv3x3_halo_kernel<BN, F16, NTAPS><<<grid, tc::HL_THREADS, smem, stream>>>(a, w, p);
 }
 
-static int tc_halo() {   // GIMMVFI_TC_HALO=0: K-poor 3x3 layers stay on the per-tap TMA path of conv_tc.cu
-  static int v = -1;
-  if (v < 0) { const char* s = getenv("GIMMVFI_TC_HALO"); v = s ? atoi(s) : 1; }
-  return v;
-}
-
 bool conv2d_halo_supported(const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out) {
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  if (!tc_halo() || in1.p || !((w.kh == 3 && w.kw == 3) || (w.kh == 1 && w.kw == 1)) || g.stride != 1 || g.reflect || w.cout > 64) return false;
+  if (in1.p || !((w.kh == 3 && w.kw == 3) || (w.kh == 1 && w.kw == 1)) || g.stride != 1 || g.reflect || w.cout > 64) return false;
   if (e.mul.p || e.gru_z.p || e.out2.p || e.split_c) return false;
   const bool h = in0.f16 != 0;
   if (h ? (!w.w_tc_h || w.cin_pad_h != 64 || in0.c > 64) : (!w.w_tc || w.cin_pad != 32 || in0.c > 32)) return false;
@@ -210,9 +204,7 @@ void conv2d_halo(Ctx& cx, const TV& in0, const ConvW& w, const ConvGeom& g, cons
   HaloParams p;
   p.tiles_x = (out.w + HL_TW - 1) / HL_TW; p.tiles_y = (out.h + HL_TH - 1) / HL_TH; p.n_img = out.n; p.H = out.h; p.W = out.w; p.cout = w.cout;
   p.origin = (g.loose_w || one) ? 0 : -1; p.round_out = out.f16 ? 0 : 1;
-  static int spin = -1;
-  if (spin < 0) { const char* s = getenv("GIMMVFI_TC_SPIN_LIMIT"); spin = s ? atoi(s) : 400; }
-  p.spin_limit = spin;
+  p.spin_limit = tc_spin_limit();
   p.bias = w.b; p.act1 = e.act1; p.slope1 = e.slope1; p.act2 = e.act2; p.slope2 = e.slope2; p.res = e.res; p.out = out;
   p.ntaps = ntaps;
   p.halo_bytes = one ? HL_TW * HL_TH * 128 : 3 * HL_COPY_BYTES;

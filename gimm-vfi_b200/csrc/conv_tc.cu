@@ -474,24 +474,11 @@ static void launch_tc(bool split, bool f16, int N, int grid, int smem, gvStream_
   else { if (f16) launch_tc_f<false, true>(N, grid, smem, stream, a0, a1, b, p); else launch_tc_f<false, false>(N, grid, smem, stream, a0, a1, b, p); }
 }
 
-static int tc_split_f16() {   // GIMMVFI_TC_SPLIT_F16=0: keep the 3xTF32 form of the split kernel
-  static int v = -1;
-  if (v < 0) { const char* s = getenv("GIMMVFI_TC_SPLIT_F16"); v = s ? atoi(s) : 1; }
-  return v;
-}
-static int tc_seg_f16() {   // K steps (of 64 elements) per tensor-core accumulation segment of the 3xF16 form
-  static int seg = -1;
-  if (seg < 0) { const char* s = getenv("GIMMVFI_TC_SEG_F16"); seg = s ? atoi(s) : 2; if (seg < 1) seg = 1; }
-  return seg;
-}
-static int tc_seg() {
-  static int seg = -1;
-  if (seg < 0) { const char* s = getenv("GIMMVFI_TC_SEG"); seg = s ? atoi(s) : 2; if (seg < 1) seg = 1; }
-  return seg;
-}
-static int tc_spin_limit() {
-  static int spin = -1;
-  if (spin < 0) { const char* s = getenv("GIMMVFI_TC_SPIN_LIMIT"); spin = s ? atoi(s) : 400; }
+// K steps (of p.bk elements) per tensor-core accumulation segment: longer segments break the fp32-class parity bar (DESIGN.md §4)
+constexpr int TC_SEG = 2;
+
+int tc_spin_limit() {
+  static const int spin = [] { const char* s = getenv("GIMMVFI_TC_SPIN_LIMIT"); return s ? atoi(s) : 400; }();
   return spin;
 }
 // pipeline depth from the shared-memory budget; returns the dynamic shared-memory size
@@ -514,7 +501,7 @@ void conv2d_tc(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const Conv
   const bool f16 = in0.f16 != 0;
   // 3xF16: the split kernel on f16 hi / lo operand pairs (two 32-channel activation boxes per 64-element K step);
   // needs pre-split weights and a first segment of whole K blocks
-  const bool sf16 = split && tc_split_f16() && w.w_tc_s != nullptr && (!in1.p || in0.c % 64 == 0);
+  const bool sf16 = split && w.w_tc_s != nullptr && (!in1.p || in0.c % 64 == 0);
   const int bk = (f16 || sf16) ? 2 * BK : BK, cin_pad = f16 ? w.cin_pad_h : (sf16 ? w.cin_pad_s : w.cin_pad);
   if (sf16) {
     cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)w.cout_pad, (cuuint64_t)(taps * 2)};
@@ -541,7 +528,7 @@ void conv2d_tc(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const Conv
   p.H = out.h; p.W = out.w; p.cout = w.cout;
   p.round_out = (split || out.f16) ? 0 : 1;   // (a half store already rounds to 10 mantissa bits)
   p.out_scale = sf16 ? 1.f / w.w_scale : 1.f;
-  p.seg = sf16 ? tc_seg_f16() : tc_seg();
+  p.seg = TC_SEG;
   p.spin_limit = tc_spin_limit();
   p.bias = w.b; p.act1 = e.act1; p.slope1 = e.slope1; p.act2 = e.act2; p.slope2 = e.slope2;
   p.res = e.res; p.mul = e.mul; p.gru_z = e.gru_z; p.gru_h = e.gru_h; p.out = out; p.out2 = e.out2; p.split_c = e.split_c;
@@ -592,7 +579,7 @@ void corr_volume_tc(Ctx& cx, const TV& fa, const float* fb_planes, const float* 
   p.taps = 1; p.kw = 1; p.ph = 0; p.pw = 0; p.stride = 1;
   p.kblocks = sf16 ? C / 64 : C / 32; p.c0_blocks = p.kblocks; p.bk = sf16 ? 2 * BK : BK;
   p.tiles_x = (fa.w + TILE_W - 1) / TILE_W; p.tiles_y = (fa.h + TILE_H - 1) / TILE_H; p.n_img = 1; p.tiles_n = tiles_n;
-  p.H = fa.h; p.W = fa.w; p.cout = NT; p.round_out = 0; p.out_scale = scale; p.seg = sf16 ? tc_seg_f16() : tc_seg();
+  p.H = fa.h; p.W = fa.w; p.cout = NT; p.round_out = 0; p.out_scale = scale; p.seg = TC_SEG;
   p.spin_limit = tc_spin_limit();
   p.bias = zero_bias; p.act1 = ACT_NONE; p.slope1 = nullptr; p.act2 = ACT_NONE; p.slope2 = nullptr;
   p.out = make_tv(vol, 1, fa.h, fa.w, NT, NT); p.out2 = TV(); p.split_c = 0;
@@ -607,7 +594,7 @@ void corr_volume_tc(Ctx& cx, const TV& fa, const float* fb_planes, const float* 
   if (cx.prof) cx.prof->end(cx.stream);
 }
 
-bool corr_volume_tc_wants_f16_planes() { return tc_split_f16() != 0; }
+bool corr_volume_tc_wants_f16_planes() { return true; }
 
 }  // namespace gv
 #endif  // GV_HOSTSIM

@@ -261,12 +261,6 @@ corr_gemm_3xf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
 }  // namespace tc
 
-static int cg_spin_limit() {
-  static int spin = -1;
-  if (spin < 0) { const char* s = getenv("GIMMVFI_TC_SPIN_LIMIT"); spin = s ? atoi(s) : 400; }
-  return spin;
-}
-
 void corr_gemm_3xf16(Ctx& cx, const void* a_planes, int64_t a_plane, int M, const void* b_planes, int64_t b_plane, int NT, int K, float scale,
                      float* vol) {
   using namespace tc;
@@ -290,7 +284,7 @@ void corr_gemm_3xf16(Ctx& cx, const void* a_planes, int64_t a_plane, int M, cons
   CgParams p;
   p.M = M; p.NT = NT; p.ksteps = K / CG_BK; p.tiles_m = (M + CG_BM - 1) / CG_BM; p.tiles_n = (NT + CG_BN - 1) / CG_BN; p.num_tiles = p.tiles_m * p.tiles_n;
   p.tma_store = (NT % 4 == 0 && aligned(vol, 16)) ? 1 : 0;
-  p.scale = scale; p.vol = vol; p.spin_limit = cg_spin_limit();
+  p.scale = scale; p.vol = vol; p.spin_limit = tc_spin_limit();
   if (p.tma_store) {
     cuuint64_t dims[2] = {(cuuint64_t)NT, (cuuint64_t)M};
     cuuint64_t str[1] = {(cuuint64_t)NT * 4};

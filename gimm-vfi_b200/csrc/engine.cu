@@ -212,11 +212,7 @@ std::string Engine::profile_json(gvStream_t stream) {
 // Engine: weights
 // ---------------------------------------------------------------------------
 Engine::Engine(int device) : device_(device) {
-  if (const char* kn = getenv("GIMMVFI_PRECISE")) precise_ = atoi(kn);   // builder experiments: override the 3xTF32 stage mask
-  if (const char* kn = getenv("GIMMVFI_HYPO_FAST")) hypo_fast_ = atoi(kn) != 0;
-  if (const char* kn = getenv("GIMMVFI_CORR_DIRECT")) corr_direct_max_t_ = atoi(kn);
   if (const char* kn = getenv("GIMMVFI_RAFT_CORR_DIRECT")) raft_direct_ = atoi(kn);            // 1: always volume-free, 0: never, unset: by size
-  if (const char* kn = getenv("GIMMVFI_GRU_HOIST")) gru_hoist_ = atoi(kn) != 0;
 #ifndef GV_HOSTSIM
   int count = 0;
   cuda_ok(cudaGetDeviceCount(&count), "cudaGetDeviceCount");
@@ -1014,7 +1010,6 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
     TV rin = r.img.batch(e0, en);
     TV raft_pad = A.tensor(en, H + 6, W + 6, 3, 4);
     pad_image4(cx, rin, raft_pad, 3);
-    if (precise_ & 32) cx.tc_split = false;   // experiment: RAFT encoders on plain TF32
     raft_encoder(N, "flow_estimator.fnet", true, rin, raft_pad, r.fmap.batch(e0, en), nullptr, nullptr, nullptr, TV(), TV());
     // the encoder's temporaries stay allocated until the caller releases the arena (bump allocator): c4 / c8 live on
     TV cin = rin, cpad = raft_pad;
@@ -1027,7 +1022,6 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
     const ConvW& wc = N.W("flow_estimator.cnet.conv2");
     TV ctx = in_order ? hx.batch(e0, en) : cb;
     raft_encoder(N, "flow_estimator.cnet", false, cin, cpad, TV(), &c4, &c8, &wc, ctx.slice(0, 128), ctx.slice(128, 128));
-    cx.tc_split = true;
     if (!in_order)
       for (int s = 0; s < S; ++s) copy_channels(cx, cb.batch(slot[src[s]], 1), hx.batch(s, 1).slice(0, 256));
     if (r.encoded) r.encoded(c4, c8, hx);
@@ -1072,7 +1066,7 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   if (r.flow_init) parallel_for(cx, (int64_t)S * 2 * h * w, FlowInitAddK{r.flow_init, coords1}, "raft_flow_init");
   TV hcur = hx.slice(0, 128), xin = hx.slice(128, 256), mot = hx.slice(256, 128);
   // iteration-invariant share of the gate convolutions (tensor-core modes; see finalize_weights), once per distinct source
-  const bool hoist = cx.tc && gru_hoist_;
+  const bool hoist = cx.tc;
   TV Pzr[2], Pq[2];
   if (hoist)
     for (int s = 0; s < 2; ++s) {
@@ -1160,7 +1154,6 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   check_problem(P);
   Net N{*this, cx};
   Arena& A = cx.arena;
-  const int knobs = precise_;   // which post-RAFT stages run in 3xTF32 (fp32-class) arithmetic: see set_precise()
   const int B = P.B, Hf = P.Hf, Wf = P.Wf, H = P.H(), W = P.W(), T = P.T;
   const int h = H / 8, w = W / 8, H4 = H / 4, W4 = W / 4;
   const bool ds = P.ds > 0.f;
@@ -1265,10 +1258,11 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   // ------------------------------------------------------------ bidirectional volume on projected features
   if (!fin && !is_f()) N.conv("amt_fproj", fmap, fproj);
   // the bidirectional volume only feeds TF32 layers (AMT update blocks) -> plain TF32 is at their input precision
-  // Few interpolated frames per pair (T <= corr_direct_max_t_): no volume at all - the lookup computes the dot products its window needs
+  // Few interpolated frames per pair (T <= corr_direct_max_t): no volume at all - the lookup computes the dot products its window needs
   // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.
   Pyramid bpyr{}; CorrFeat bfeat{};
-  const bool corr_direct = tc_mode_ >= 1 && T <= corr_direct_max_t_ && fproj.c == 256 && h >= 16 && w >= 16;
+  constexpr int corr_direct_max_t = 2;
+  const bool corr_direct = tc_mode_ >= 1 && T <= corr_direct_max_t && fproj.c == 256 && h >= 16 && w >= 16;
   if (corr_direct) {
     TV Fl = fproj;
     bfeat.c = 256; bfeat.scale = 1.0f / std::sqrt((float)fproj.c);
@@ -1326,7 +1320,6 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     float* sc = A.alloc_f((size_t)absmax_scratch_floats(f01));
     absmax_per_sample(cx, f01, f10, scaler, sc);
   }
-  flow_absmax_ = scaler;   // per-sample max |flow| over both directions: also bounds the forward splat's reach (gimm_decode)
   TV nf = A.tensor(2 * B, H, W, 2);
   normalize_flow_pair(cx, f01, f10, scaler, nf.batch(0, B), nf.batch(B, B));
   if (io.nflow)
@@ -1334,9 +1327,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       nhwc_to_nchw(cx, nf.batch(j * B, B), io.nflow + (int64_t)j * H * W, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
   TV wts = A.tensor(2 * B, H, W, 1);
   TV X64 = A.tensor(B, H, W, 64);   // [lat0 | lat1 | splat0 | splat1]
-  cx.tc_split = (knobs & 1) != 0;
   gimm_encode(N, nf, f01, f10, wts, X64);
-  cx.tc_split = false;
 
   // ------------------------------------------------------------ per-timestep: GIMM decode + frame synthesis
   TV grid_flow = A.tensor(B, h, w, 4);   // flow_4_lr = cat(fl0, fl1)
@@ -1347,9 +1338,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     const bool last = ti == T - 1;
     const float* tdev = io.t + (int64_t)ti * B;
     TV ninr = A.tensor(B, H, W, 2);
-    cx.tc_split = (knobs & 1) != 0;
     gimm_decode(N, X64, f01, f10, wts, tdev, io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3, ninr, last);
-    cx.tc_split = (knobs & 4) != 0;   // init decoder + update blocks
     if (io.ninrflow) nhwc_to_nchw(cx, ninr, io.ninrflow + (int64_t)ti * B * 2 * H * W, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
     TV flow_t = A.tensor(B, H, W, 2);
     unnormalize_flow(cx, ninr, scaler, flow_t);
@@ -1421,7 +1410,6 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
     if (io.flowt1_4) nhwc_to_nchw(cx, fl4.slice(2, 2), io.flowt1_4 + (int64_t)ti * B * 2 * H4 * W4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
 
     // NewMultiFlowDecoder (fi_components.py:307-340)
-    cx.tc_split = (knobs & 8) != 0;
     TV F0 = A.tensor(B, H, W, 6, 8), F1 = A.tensor(B, H, W, 6, 8), Mk = A.tensor(B, H, W, 3, 4), Rs = A.tensor(B, H, W, 9, 12);
     // debug snapshots of the concat, the fp32 flows / mask and convblock.4's output: allocated here, outside the block that frees them
     const bool snap = debug_ && last;
@@ -1452,7 +1440,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       }
       // precision mode 3: the 256-channel residual trunk (9 of the 10 heaviest launches) is stored in fp16 and runs on the
       // f16 tensor-core path (same 10-bit mantissa as TF32, half the bytes per operand, twice the MMA rate)
-      TV x1 = (cx.tc && tc_mode_ >= 3 && !(knobs & 8)) ? A.tensor_h(B, H, W, 256) : A.tensor(B, H, W, 256);
+      TV x1 = (cx.tc && tc_mode_ >= 3) ? A.tensor_h(B, H, W, 256) : A.tensor(B, H, W, 256);
       N.convrelu("amt_final_decoder.convblock.0", fin1, x1);
       for (int k = 1; k <= 3; ++k) resblock(N, "amt_final_decoder.convblock." + std::to_string(k), x1, 256, 64);
       TV o24 = A.tensor(B, H, W, 24);
@@ -1462,7 +1450,6 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       A.release(mk);
     }
     if (last) { tap("syn.F0", F0); tap("syn.F1", F1); tap("syn.Mk", Mk); tap("syn.Rs", Rs); }
-    cx.tc_split = (knobs & 16) != 0;   // comb block
     TV F0f = F0, F1f = F1, Mkf = Mk, Rsf = Rs;
     if (ds) {  // gimmvfi_r.py:294-303
       F0f = A.tensor(B, Hf, Wf, 6, 8); F1f = A.tensor(B, Hf, Wf, 6, 8); Mkf = A.tensor(B, Hf, Wf, 3, 4); Rsf = A.tensor(B, Hf, Wf, 9, 12);
@@ -1486,7 +1473,6 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       combine_output(cx, mean3, c3, io.imgt_pred + (int64_t)ti * B * 3 * Hf * Wf);
       if (last) { tap("syn.w9", w9); tap("syn.mean3", mean3); tap("syn.c3", c3); }
     }
-    cx.tc_split = false;
   }
 }
 
@@ -1528,18 +1514,14 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
   Ctx& cx = N.cx; Arena& A = cx.arena;
   const int B = f01.n, H = f01.h, W = f01.w;
   const size_t mk0 = A.mark();
-  // ---- forward splat of both latents to time t (gimmvfi_r.py:171-193)
-  // one pass per direction (target tiles in shared memory, bounded by the per-sample max |flow|); else memset + vector reductions + normalise
-  // (the one-pass kernel is the linear mode's; softmax and sum take the vector-reduction form)
+  // ---- forward splat of both latents to time t (gimmvfi_r.py:171-193): memset + vector reductions + normalise (the one-pass
+  // softsplat_fused is slower: its shared-memory atomics are compare-and-swap loops, DESIGN.md §3.5)
   const int fwarp = motion_.fwarp;
-  const bool one_pass = fwarp == SPLAT_LINEAR && flow_absmax_ != nullptr &&
-                        softsplat_fused(cx, X64.slice(0, 16), f01, wts.batch(0, B), tdev, 0, flow_absmax_, X64.slice(32, 16)) &&
-                        softsplat_fused(cx, X64.slice(16, 16), f10, wts.batch(B, B), tdev, 1, flow_absmax_, X64.slice(48, 16));
-  if (!one_pass && fwarp == SPLAT_SUM) {   // the plain sum is the result: accumulated straight into the latent buffer
+  if (fwarp == SPLAT_SUM) {   // the plain sum is the result: accumulated straight into the latent buffer
     fill(cx, X64.slice(32, 32), 0.f);
     softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, wts.batch(0, B), tdev, 0, X64.slice(32, 16), SPLAT_SUM);
     softsplat_accumulate_mode(cx, X64.slice(16, 16), f10, wts.batch(B, B), tdev, 1, X64.slice(48, 16), SPLAT_SUM);
-  } else if (!one_pass) {
+  } else {
     TV acc = A.tensor(2 * B, H, W, 17, 20);
     if (!cx.dry) dev_memset(acc.p, 0, (size_t)2 * B * H * W * 20 * sizeof(float), cx.stream);
     softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, wts.batch(0, B), tdev, 0, acc.batch(0, B), fwarp);
@@ -1551,13 +1533,12 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
   // HypoNet (hyponet.py:71-146).  Tensor-core modes: ONE fused kernel (hyponet.cu) that takes the refined latent and the caller's
   // coordinate tensor directly; fp32 mode: five 1x1 convolutions on a packed [latent32 | t,y,x] input.
   // The coordinate grid (Hc, Wc) = ninr's size may differ from the flow resolution (GIMM standalone): HypoNet first resizes the
-  // latent to the grid (hyponet.py:86-90).  The fp32-class kernel does that in its layer 0 (hyponet_fused3_resample); the other
-  // paths resize the refined latent into their grid-sized input.
+  // latent to the grid (hyponet.py:86-90).  The fused kernel does that in its layer 0 (hyponet_fused3_resample); fp32 mode resizes
+  // the refined latent into its grid-sized input.
   const int Hc = ninr.h, Wc = ninr.w;
   const bool same = Hc == H && Wc == W;
-  const bool fused = cx.tc && hypo_blob_ != nullptr && !(precise_ & 2);
-  const bool resample_in_kernel = !same && fused && !hypo_fast_;
-  const bool split_saved = cx.tc_split;
+  const bool fused = cx.tc && hypo_blob_ != nullptr;
+  const bool resample_in_kernel = !same && fused;
   TV hin = resample_in_kernel ? TV() : fused ? A.tensor(B, Hc, Wc, 32) : A.tensor(B, Hc, Wc, 35, 36);
   TV lat = same ? hin.slice(0, 32) : A.tensor(B, H, W, 32);   // the refined latent, at the flow resolution
   {
@@ -1579,12 +1560,10 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
   if (resample_in_kernel) {
     hyponet_fused3_resample_act(cx, lat, coords_t, hypo_blob3_, ninr, act, w0);
   } else if (fused) {
-    // fp32-class by default: the flow is (2 o - 1) * max|flow|, so operand rounding at 2^-11 becomes ~1e-2 px at 40 px motion and
-    // moves real frames by > 1e-3 (tests/test_bench_parity_gpu.py, demo frames); hypo_fast_ selects the TF32 / half-operand kernel
-    if (hypo_fast_) hyponet_fused_act(cx, hin, coords_t, hypo_blob_, ninr, act, w0);
-    else hyponet_fused3_act(cx, hin, coords_t, hypo_blob3_, ninr, act, w0);
+    // fp32-class: the flow is (2 o - 1) * max|flow|, so operand rounding at 2^-11 becomes ~1e-2 px at 40 px motion and
+    // moves real frames by > 1e-3 (tests/test_bench_parity_gpu.py, demo frames)
+    hyponet_fused3_act(cx, hin, coords_t, hypo_blob3_, ninr, act, w0);
   } else {
-    cx.tc_split = (precise_ & 2) != 0;
     hypo_pack_input(cx, coords_t, hin.slice(32, 3));
     const size_t mk = A.mark();
     TV a = A.tensor(B, Hc, Wc, 128), b = A.tensor(B, Hc, Wc, 128);
@@ -1601,7 +1580,6 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
     }
     N.conv("hyponet.params_dict.linear_wb4", b, ninr);
     A.release(mk);
-    cx.tc_split = split_saved;
   }
   if (!debug_) A.release(mk0);   // (debug taps keep pointing into this region)
 }
@@ -1635,12 +1613,6 @@ void Engine::run_gimm(Ctx& cx, const Problem& P, const GimmIO& io) {
   TV f01 = fl.batch(0, B), f10 = fl.batch(B, B);
   TV wts = A.tensor(2 * B, H, W, 1);
   TV X64 = A.tensor(B, H, W, 64);
-  {   // bound of the splat's reach (the caller's normalisation scale is not passed in: recompute max |ori_flow| per sample)
-    float* amax = A.alloc_f(std::max(B, 64));
-    float* sc = A.alloc_f((size_t)absmax_scratch_floats(f01));
-    absmax_per_sample(cx, f01, f10, amax, sc);
-    flow_absmax_ = amax;
-  }
   gimm_encode(N, nf, f01, f10, wts, X64);
   TV ninr = A.tensor(B, Hc, Wc, 2);
   for (int ti = 0; ti < T; ++ti) {
@@ -1737,8 +1709,8 @@ void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t wor
     // (the legacy default stream - handles 0 / 1 / 2 - cannot be captured: such callers run eagerly)
     if (use_graph_ && !profile_ && !debug_ && fc_ == nullptr && reinterpret_cast<uintptr_t>(stream) > 2) {
       // everything a recorded launch sequence depends on: problem, every caller pointer, the workspace, the arithmetic mode, the weights
-      std::vector<uint64_t> key = {(uint64_t)p.B, (uint64_t)p.Hf, (uint64_t)p.Wf, (uint64_t)p.T, (uint64_t)p.Hc, (uint64_t)p.Wc, 0, (uint64_t)tc_mode_, (uint64_t)precise_,
-                                   (uint64_t)hypo_fast_, (uint64_t)(raft_direct_ + 2), (uint64_t)corr_direct_max_t_, (uint64_t)gru_hoist_, (uint64_t)weights_version_, (uint64_t)raft_iters, (uint64_t)workspace, (uint64_t)workspace_bytes, (uint64_t)(uintptr_t)stream};
+      std::vector<uint64_t> key = {(uint64_t)p.B, (uint64_t)p.Hf, (uint64_t)p.Wf, (uint64_t)p.T, (uint64_t)p.Hc, (uint64_t)p.Wc, 0, (uint64_t)tc_mode_,
+                                   (uint64_t)(raft_direct_ + 2), (uint64_t)weights_version_, (uint64_t)raft_iters, (uint64_t)workspace, (uint64_t)workspace_bytes, (uint64_t)(uintptr_t)stream};
       std::memcpy(&key[6], &p.ds, sizeof(float));
       const void* ptrs[] = {io.img_xs, io.coords, io.t, io.imgt_pred, io.img_warp_4, io.flowt0_1, io.flowt1_1, io.flowt0_4, io.flowt1_4, io.raft_flow, io.nflow, io.ninrflow, io.flowt};
       for (const void* q : ptrs) key.push_back((uint64_t)(uintptr_t)q);

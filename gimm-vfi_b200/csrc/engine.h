@@ -179,13 +179,14 @@ class Engine {
   void set_debug(bool on) { debug_ = on; }
   // per-kernel CUDA-event timing of the next forward(s): {"name": {"ms", "work", "launches"}}
   void set_profile(bool on) { profile_ = on; }
-  // 0: fp32 CUDA cores everywhere; 1: post-RAFT convs on TF32 tensor cores; 2: + RAFT convs on 3xTF32 tensor cores;
-  // 3: + final-decoder residual trunk in fp16; 4: + the 32/64-channel full-resolution chains in fp16 (experimental)
+  // 0: fp32 CUDA cores everywhere; 1: post-RAFT convs on TF32 tensor cores; 2: + RAFT convs on fp32-class (3xF16) tensor cores;
+  // 3: + final-decoder residual trunk in fp16; 4: + the 32/64-channel full-resolution chains in fp16 (the default of GIMM-VFI-R / -F,
+  // RAFT and FlowFormer)
   void set_tensor_cores(int mode) { tc_mode_ = mode; }
   // the motion settings the next finalize_weights* packs the weights for and the forwards after it run with
   void set_motion_config(const MotionConfig& m) { motion_next_ = m; }
   const MotionConfig& motion() const { return motion_; }
-  // precision mode 4 (experimental, see DESIGN.md): the 32/64-channel full-resolution chains (motion encoder laterals, latent
+  // precision mode 4 (see DESIGN.md): the 32/64-channel full-resolution chains (motion encoder laterals, latent
   // refiner, final-decoder upsample branch) are stored in half precision like the residual trunk of mode 3
   bool half_chains(const Ctx& cx) const { return cx.tc && tc_mode_ >= 4; }
   std::string profile_json(gvStream_t stream);
@@ -258,7 +259,6 @@ class Engine {
   struct GraphEntry { std::vector<uint64_t> key; void* exec = nullptr; int64_t launches = 0; int seen = 0; };
   std::vector<GraphEntry> graphs_;
   void clear_graphs();
-  int precise_ = 0;   // bit mask of post-RAFT stages in 3xTF32: 1 GIMM encoders / latent refiner, 2 HypoNet, 4 init decoder + update blocks, 8 final decoder, 16 combine
   std::vector<float> ff_c1w_, ff_c1b_;
   float* fc_ = nullptr; size_t fc_bytes_ = 0; bool fc_load_ = false, fc_store_ = false;
   // what the cache holds (host-side bookkeeping of the last store): a load with a different buffer / problem is refused
@@ -277,14 +277,10 @@ class Engine {
   std::map<std::string, const float*> vec_;
   std::vector<void*> dev_allocs_;
   std::map<std::string, TV> taps_;
-  const float* flow_absmax_ = nullptr;   // device, per sample: max |flow| over both directions of the forward in flight
   const void* hypo_blob_ = nullptr;   // packed parameters of the fused HypoNet kernel (common.h hypo::)
-  const void* hypo_blob3_ = nullptr;  // ... of its fp32-class variant (common.h hypo3::), the default
-  bool hypo_fast_ = false;            // true: TF32 / half-operand HypoNet kernel (0.56 ms vs the fp32-class one; fails the 1e-3 bound on real frames)
-  bool gru_hoist_ = true;             // SepConvGRU: the context input's share of the gate convolutions is computed once per pair (GIMMVFI_GRU_HOIST=0: every iteration)
+  const void* hypo_blob3_ = nullptr;  // ... of its fp32-class variant (common.h hypo3::), the one the forwards run
   int raft_direct_ = -1;              // RAFT's own lookups without a volume: -1 = when the volume pyramid exceeds raft_direct_auto_bytes_ (GIMMVFI_RAFT_CORR_DIRECT)
   double raft_direct_auto_bytes_ = 32e9;   // set to 0.4 x the device memory by the constructor (GIMMVFI_RAFT_CORR_DIRECT_GB overrides)
-  int corr_direct_max_t_ = 2;         // BidirCorrBlock: volume-free lookup when a pair is interpolated at <= this many timesteps (GIMMVFI_CORR_DIRECT; 0: always the volume)
   const float* g9_ = nullptr; const float* alpha_fe_ = nullptr; const float* alpha_v_ = nullptr;
   MotionConfig motion_next_;   // set_motion_config
   MotionConfig motion_;        // what the packed HypoNet weights were built with (finalize_gimm_part); the forwards read this one

@@ -522,7 +522,7 @@ void Engine::run_flowformer(Ctx& cx, Net& N, const TV& img, const std::vector<in
      agg = A.tensor(S, h, w, 128), zb = A.tensor(S, h, w, 128), rh = A.tensor(S, h, w, 128), fh = A.tensor(S, h, w, 256), mask = A.tensor(S, h, w, 576);
   init_coords(cx, coords1);
   if (flow_init) parallel_for(cx, (int64_t)S * 2 * h * w, FlowInitAddK{flow_init, coords1}, "flowformer_flow_init");   // decoder.py:265-267
-  const bool hoist = cx.tc && gru_hoist_;
+  const bool hoist = cx.tc;
   TV Pzr[2], Pq[2];
   if (hoist)
     for (int sx = 0; sx < 2; ++sx) {

@@ -7,7 +7,6 @@ namespace gv {
 
 struct Net {
   Engine& E; Ctx& cx;
-  bool small_cout7_ = getenv("GIMMVFI_CONV7_SMALL") ? atoi(getenv("GIMMVFI_CONV7_SMALL")) != 0 : true;
   const ConvW& W(const std::string& n) const {
     auto it = E.conv_.find(n);
     if (it == E.conv_.end()) throw std::runtime_error("gimmvfi: conv '" + n + "' not packed");
@@ -41,7 +40,7 @@ struct Net {
   }
   // 7x7 conv on few channels through the x-packed weights: zero-padded copy of `in`, then a (7 x 1) conv over 7*ldp lanes
   void conv7x(const std::string& name, const TV& in, const TV& out, int act = ACT_NONE, const float* slope = nullptr) {
-    if (small_cout7_ && conv7x7_small_cout(cx, in, W(name), act, slope, out)) return;   // <= 4 output channels: exact fp32 shared-memory kernel (conv.cu)
+    if (conv7x7_small_cout(cx, in, W(name), act, slope, out)) return;   // <= 4 output channels: exact fp32 shared-memory kernel (conv.cu)
     const ConvW& w = W(name + "#xp");
     const int k = w.kh, ldp = w.cin / k;   // (k x k kernel packed as k x 1 over k * ldp lanes)
     Arena& A = cx.arena;

@@ -1077,15 +1077,11 @@ __global__ void __launch_bounds__(256) softsplat_tile_kernel(TV lat, TV flow, TV
   }
 }
 #endif
-// fused splat: returns false when the layout does not qualify (caller falls back to memset + accumulate + normalise)
+// fused splat: returns false when the layout does not qualify
 bool softsplat_fused(Ctx& cx, const TV& lat, const TV& flow, const TV& metric, const float* t_per_sample, int t_mode, const float* flow_absmax,
-                     const TV& out, bool force) {
+                     const TV& out) {
 #ifndef GV_HOSTSIM
-  static int on = -1;
-  // off by default: fp32 (and 64-bit integer) atomic adds on SHARED memory are compare-and-swap loops, while the three-pass form's
-  // red.global.add.v4.f32 run in the L2 atomic units
-  if (on < 0) { const char* s = getenv("GIMMVFI_SPLAT_TILE"); on = s ? atoi(s) : 0; }
-  if ((!on && !force) || !flow_absmax || lat.c != 16 || out.c != 16 || !vec4_ok(lat) || !vec4_ok(out) || (reinterpret_cast<uintptr_t>(flow.p) & 7) || flow.ld % 2 || flow.sn % 2 ||
+  if (!flow_absmax || lat.c != 16 || out.c != 16 || !vec4_ok(lat) || !vec4_ok(out) || (reinterpret_cast<uintptr_t>(flow.p) & 7) || flow.ld % 2 || flow.sn % 2 ||
       flow.f16 || metric.f16)
     return false;
   if (cx.dry) return true;

@@ -57,23 +57,6 @@ def test_gimm_on_grid_matches_reference_golden(name, mode, weights0):
     assert one.shape == (B, 1, Hc, Wc, 2)
 
 
-@pytest.mark.parametrize("env", ["GIMMVFI_HYPO_FAST=1", "GIMMVFI_PRECISE=2"])
-def test_gimm_on_grid_other_hyponet_paths(env, weights0, monkeypatch):
-    """The TF32 / half-operand HypoNet kernel and the 3xTF32 convolution HypoNet take the latent resized into their grid-sized input
-    (the engine reads these switches when it is created)."""
-    k, v = env.split("=")
-    monkeypatch.setenv(k, v)
-    name = "gimm_grid_64x96_r2_t0.25_0.75"
-    meta = MANIFEST[name]
-    g = load_golden(name)
-    out, _ = _run_fixture(_gimm(weights0, 1), meta)
-    tol = 5e-3   # TF32 convolutions; the fast HypoNet's half operands stay inside this bar on these flows
-    for i in range(len(meta["timesteps"])):
-        err = np.abs(out[i].cpu().numpy() - g["out_%d" % i]).max()
-        print(env, "max err %.3e" % err)
-        assert err <= tol
-
-
 def test_gimm_list_form_with_two_grid_sizes(weights0):
     B, H, W = 1, 64, 96
     m = _gimm(weights0, 0)
