@@ -5,14 +5,18 @@
 // 3x3 layer whose distinct input is 23 KB, plus the weight boxes.  Here a tile costs 54 KB of TMA traffic and no weight traffic.
 //
 // How: output tile = 8 (x) x 16 (y) pixels, so the 8-row groups of the M = 128 operand are image rows.  Three TMA boxes
-// {K, 8 x, 18 y} land the tile's columns shifted by kx = 0, 1, 2 (with the halo rows) 128B-swizzled in shared memory, each 18 KB =
-// a whole number of 1024-byte swizzle atoms; tap (ky, kx) is then the operand descriptor of copy kx started ky image rows (= ky atoms)
-// further, so every descriptor start is 1024-byte aligned and the canonical K-major SWIZZLE_128B layout holds for every tap.
-// Out-of-bounds box elements are zero-filled = the convolution's zero padding.  1x1 layers load the 8 x 16 tile itself (one tap).
+// {K, 8 x, 18 y} land the tile's columns shifted by kx = 0, 1, 2 (with the halo rows) swizzled in shared memory, each a whole number
+// of swizzle atoms; tap (ky, kx) is then the operand descriptor of copy kx started ky image rows (= ky atoms) further, so every
+// descriptor start is atom-aligned and the canonical K-major swizzled layout holds for every tap.  K rows are 128 bytes (SWIZZLE_128B,
+// 18 KB per copy), or 64 bytes (SWIZZLE_64B, 9 KB per copy) when the input's channels fit: 32 half / 16 fp32 channels then take half
+// the MMAs and half the stage.  Out-of-bounds box elements are zero-filled = the convolution's zero padding.  1x1 layers load the
+// 8 x 16 tile itself (one tap).
 //
-// Roles: warp 8 TMA producer (weights once, then one stage per tile), warpgroups 0 / 1 the MMAs of image rows 0-7 / 8-15 of the tile
-// and their epilogue straight from the accumulator registers: a thread holds two pixels (one column, two rows) x BN / 4 channels as
-// channel pairs; the four threads of a quad write 8 consecutive channels = 32 contiguous bytes of the NHWC output.
+// Roles: warp 8 TMA producer (weights once, then one stage per tile); with 32 output channels warpgroups 0 / 1 alternate whole tiles
+// (two m64 accumulators: image rows 0-7 / 8-15), so one warpgroup's epilogue runs under the other's MMAs; with 64 they take image
+// rows 0-7 / 8-15 of every tile.  The epilogue stages the raw accumulators per warp in shared
+// memory and runs over 8-channel pieces of whole pixels (16- or 32-byte stores of the NHWC output), reading each piece's residual
+// one piece ahead, the first while the MMAs run.
 #include "common.h"
 
 #ifndef GV_HOSTSIM
@@ -26,56 +30,57 @@ namespace tc {
 
 constexpr int HL_TW = 8, HL_TH = 16;                  // output tile (x, y)
 constexpr int HL_BH = HL_TH + 2;                      // halo rows
-constexpr int HL_COPY_BYTES = HL_TW * HL_BH * 128;    // one x-shifted copy: 18 KB
-constexpr int HL_MAX_STAGES = 4;
+constexpr int HL_MAX_STAGES = 6;
 constexpr int HL_THREADS = 256 + 32;
 
 struct HaloParams {
   int tiles_x, tiles_y, n_img, H, W, cout, stages, origin, round_out, spin_limit;
   int halo_bytes;   // bytes of one pipeline stage (multiple of 1024)
-  int ntaps;        // 9 (3x3) or 1 (1x1)
+  int stg_ld;       // bytes per pixel of the accumulator staging (BN fp32 channels + 16 bytes of bank offset)
   const float* bias; int act1; const float* slope1; int act2; const float* slope2;
   TV res, out;
 };
 
-// 2 channels (c, c + 1) of an fp32 or half tensor at element offset eoff; channels >= cout read as 0 / are not written
-__device__ __forceinline__ void load2_any(const TV& t, int64_t eoff, int c, int cout, float* r) {
-  if (t.f16) {
-    const __half* q = reinterpret_cast<const __half*>(t.p) + eoff;
-    r[0] = __half2float(q[0]); r[1] = c + 1 < cout ? __half2float(q[1]) : 0.f;
-  } else {
-    r[0] = t.p[eoff]; r[1] = c + 1 < cout ? t.p[eoff + 1] : 0.f;
-  }
-}
-__device__ __forceinline__ void store2(const TV& t, int64_t eoff, const float* o, int c, int cout) {
-  const bool two = c + 1 < cout;
-  if (t.f16) {
-    __half* q = reinterpret_cast<__half*>(t.p) + eoff;
-    const float a = fminf(fmaxf(o[0], -65504.f), 65504.f), b = fminf(fmaxf(o[1], -65504.f), 65504.f);
-    if (two && (reinterpret_cast<uintptr_t>(q) & 3) == 0) *reinterpret_cast<__half2*>(q) = __floats2half2_rn(a, b);
-    else { q[0] = __float2half_rn(a); if (two) q[1] = __float2half_rn(b); }
-  } else {
-    float* q = t.p + eoff;
-    if (two && (reinterpret_cast<uintptr_t>(q) & 7) == 0) *reinterpret_cast<float2*>(q) = make_float2(o[0], o[1]);
-    else { q[0] = o[0]; if (two) q[1] = o[1]; }
+// K-major operand descriptor of rows of RB bytes: SWIZZLE_128B (RB = 128) or SWIZZLE_64B (RB = 64); 8-row atoms of 8 RB bytes (SBO)
+template <int RB>
+__device__ __forceinline__ uint64_t halo_desc(uint32_t saddr) {
+  if constexpr (RB == 128) return make_smem_desc(saddr);
+  else {
+    static_assert(RB == 64, "RB");
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;   // layout type 2 = SWIZZLE_64B
+    return d;
   }
 }
 
-// BN: output channels (32 / 64), F16: half operands, NTAPS: 9 or 1 - all compile-time, so the MMA chain of a tile is straight-line
-// code whose accumulators stay in fixed registers (no serialising register moves between the asynchronous MMAs)
-template <int BN, bool F16, int NTAPS>
+// BN: output channels (32 / 64), F16: half operands, NTAPS: 9 or 1, RB: bytes of K per operand row (128, or 64 when the input's
+// channels fit in 64 bytes: 32 half / 16 fp32 channels) - all compile-time, so the MMA chain of a tile is straight-line code whose
+// accumulators stay in fixed registers (no serialising register moves between the asynchronous MMAs)
+template <int BN, bool F16, int NTAPS, int RB>
 __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                                                                     const __grid_constant__ HaloParams p) {
+  constexpr int KSTEPS = RB / 32;                 // 32 bytes of K per MMA (8 tf32 / 16 half)
+  constexpr int COPY = HL_TW * HL_BH * RB;        // one x-shifted copy: a whole number of 1024-byte blocks
+  constexpr int ROW = HL_TW * RB;                 // one image row of the tile = 8 operand rows = one swizzle atom
+  // BN = 32: each warpgroup owns whole tiles (two m64 accumulators, image rows 0-7 / 8-15), so one warpgroup's epilogue runs under the
+  // other's MMAs.  BN = 64: the two warpgroups split each tile (image rows 0-7 / 8-15): owning whole 64-channel tiles measured up to
+  // 1.4x slower on these layers, the epilogue of a whole tile on 4 warps outlasting the other warpgroup's MMAs.
+  constexpr bool OWN = BN == 32;
+  constexpr int NH = OWN ? 2 : 1;                 // m64 halves of a tile per warpgroup
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int w_bytes = NTAPS * BN * 128;
+  const int w_bytes = NTAPS * BN * RB;
   const int w_region = (w_bytes + 1023) & ~1023;
   uint8_t* wsm = smem;
   uint8_t* halo = smem + w_region;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(halo + p.stages * p.halo_bytes);
+  uint8_t* stg_all = halo + p.stages * p.halo_bytes;   // [8 warps][NH x 16 pixels][stg_ld bytes]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_all + 8 * NH * 16 * p.stg_ld);
   uint64_t* w_bar = bars;                          // weights landed
   uint64_t* full_bar = bars + 1;                   // [HL_MAX_STAGES]
-  uint64_t* empty_bar = bars + 1 + HL_MAX_STAGES;  // [HL_MAX_STAGES]  the 8 consumer warps are done with the stage
+  uint64_t* empty_bar = bars + 1 + HL_MAX_STAGES;  // [HL_MAX_STAGES]  the consuming warps (4, or 8 when the warpgroups split a tile) are done
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.n_img * p.tiles_y * p.tiles_x;
   const int SPIN = p.spin_limit;
@@ -84,15 +89,18 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
     mbar_init(w_bar, 1);
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], OWN ? 4 : 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
+  // The CTA's i-th tile (tile blockIdx.x + i * gridDim.x) goes through stage i % stages, fill (i / stages); with OWN warpgroup i % 2
+  // consumes it (the empty barrier counts that warpgroup's 4 warps), otherwise both do (8 warps).  Both sides derive the phase of fill
+  // i from i alone.
   if (warp == 8) {
     if (elect_one()) {
       mbar_expect_tx(w_bar, (uint32_t)w_bytes);
-      tma_load_3d(wsm, &tmW, w_bar, 0, 0, 0);   // {K block, BN rows, taps}
+      tma_load_3d(wsm, &tmW, w_bar, 0, 0, 0);   // {K, BN rows, taps}
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int r = tile; const int tx = r % p.tiles_x; r /= p.tiles_x; const int ty = r % p.tiles_y; const int n = r / p.tiles_y;
@@ -100,7 +108,7 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
         mbar_expect_tx(&full_bar[stage], (uint32_t)p.halo_bytes);
         const int ncopies = NTAPS == 9 ? 3 : 1;
         for (int kx = 0; kx < ncopies; ++kx)
-          tma_load_4d(halo + stage * p.halo_bytes + kx * HL_COPY_BYTES, &tmA, &full_bar[stage], 0, tx * HL_TW + p.origin + kx, ty * HL_TH + p.origin, n);
+          tma_load_4d(halo + stage * p.halo_bytes + kx * COPY, &tmA, &full_bar[stage], 0, tx * HL_TW + p.origin + kx, ty * HL_TH + p.origin, n);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
     }
@@ -108,61 +116,139 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
   }
 
   const int wg = warp >> 2, wq = warp & 3, gid = lane >> 2, tig = lane & 3;
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  uint8_t* stg = stg_all + warp * NH * 16 * p.stg_ld;
+  float acc[NH][BN / 2];
   mbar_wait(w_bar, 0, SPIN);
   const uint32_t w_s = smem_u32(wsm);
-  int stage = 0; uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  for (int i = OWN ? wg : 0;; i += OWN ? 2 : 1) {
+    const int tile = blockIdx.x + i * gridDim.x;
+    if (tile >= num_tiles) break;
+    const int stage = i % p.stages;
+    const uint32_t phase = (uint32_t)(i / p.stages) & 1u;
     int r = tile; const int tx = r % p.tiles_x; r /= p.tiles_x; const int ty = r % p.tiles_y; const int n = r / p.tiles_y;
     mbar_wait(&full_bar[stage], phase, SPIN);
-    const uint32_t h_s = smem_u32(halo + stage * p.halo_bytes) + (uint32_t)(wg * 64 * 128);   // this warpgroup's 8 image rows
+    const uint32_t h_s = smem_u32(halo + stage * p.halo_bytes);
     wgmma_fence();
 #pragma unroll
     for (int tap = 0; tap < NTAPS; ++tap) {
       const int ky = tap / 3, kx = tap % 3;
-      const uint64_t ad = make_smem_desc(h_s + (uint32_t)(kx * HL_COPY_BYTES + ky * HL_TW * 128));   // copy kx, image row ky
-      const uint64_t bd = make_smem_desc(w_s + (uint32_t)(tap * BN * 128));
+      const uint64_t bd = halo_desc<RB>(w_s + (uint32_t)(tap * BN * RB));
 #pragma unroll
-      for (int k = 0; k < 4; ++k)   // 32 bytes of K per MMA (8 tf32 / 16 half); channels beyond cin are TMA zero fill on both operands
-        wgmma_ss<BN, F16>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (tap | k) ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence<BN / 2>(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[stage]);   // the producer refills the stage while this warp runs the epilogue
-    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-    // ---- epilogue: rows gid / gid + 8 of the warp's 16 = pixel column gid of image rows y0, y0 + 1
-    const int x = tx * HL_TW + gid, y0 = ty * HL_TH + wg * 8 + wq * 2;
+      for (int h = 0; h < NH; ++h) {   // copy kx, image row 8 (h + wg) + ky or 8 h + ky
+        const uint64_t ad = halo_desc<RB>(h_s + (uint32_t)(kx * COPY + (8 * (OWN ? h : wg) + ky) * ROW));
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = 8 * j + 2 * tig;
-      if (c >= p.cout) break;
-      const float b0 = __ldg(p.bias + c), b1 = __ldg(p.bias + c + 1);   // (bias padded past cout)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int y = y0 + h;
-        if (y >= p.H || x >= p.W) continue;
-        float o[2] = {acc[4 * j + 2 * h] + b0, acc[4 * j + 2 * h + 1] + b1};
-        act_n<2>(o, p.act1, p.slope1, c, p.cout);
-        if (p.res.p) { float t[2]; load2_any(p.res, p.res.off(n, y, x) + c, c, p.cout, t); o[0] += t[0]; o[1] += t[1]; }
-        if (p.act2 != ACT_NONE) act_n<2>(o, p.act2, p.slope2, c, p.cout);
-        if (p.round_out) { o[0] = rn_tf32(o[0]); o[1] = rn_tf32(o[1]); }
-        store2(p.out, p.out.off(n, y, x) + c, o, c, p.cout);
+        for (int k = 0; k < KSTEPS; ++k)   // channels beyond cin are TMA zero fill on both operands
+          wgmma_ss<BN, F16>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (tap | k) ? 1u : 0u);
       }
     }
+    wgmma_commit();
+    // The epilogue works on 8-channel pieces of whole pixels: the warp's NH x 16 pixels (image rows 8 h + 2 wq, + 1 with OWN, else
+    // 8 wg + 2 wq, + 1; columns 0-7) x BN channels.  A runtime loop over the pieces keeps ONE copy of the activation code: unrolled
+    // over the accumulator pairs it was ~5k instructions per kernel, the epilogue bound by instruction fetch.  The residual of the
+    // lane's next piece is read before the current piece is computed, the first one while the MMAs run.
+    constexpr int CPP = BN / 8;            // pieces per pixel
+    constexpr int NPC = NH * 16 * CPP;     // pieces per warp and tile (a multiple of 32)
+    const int yw = ty * HL_TH + (OWN ? 0 : 8 * wg) + wq * 2;
+    auto piece = [&](int q, int& px, int& py, int& c0) {
+      const int pix = q / CPP;
+      px = tx * HL_TW + (pix & 7); py = yw + 8 * (pix >> 4) + ((pix >> 3) & 1); c0 = (q % CPP) * 8;
+      return px < p.W && py < p.H && c0 < p.cout;
+    };
+    // the residual of piece q as raw storage bits (8 halves in r[0], or 8 floats in r[0], r[1])
+    auto load_res = [&](int q, uint4* rr) {
+      int px, py, c0;
+      rr[0] = rr[1] = make_uint4(0u, 0u, 0u, 0u);
+      if (!piece(q, px, py, c0)) return;
+      const int64_t e = p.res.off(n, py, px) + c0;
+      if (p.res.f16) {
+        const __half* src = reinterpret_cast<const __half*>(p.res.p) + e;
+        if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) rr[0] = *reinterpret_cast<const uint4*>(src);
+        else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<__half*>(rr)[u] = src[u];
+      } else {
+        const float* src = p.res.p + e;
+        if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) { rr[0] = *reinterpret_cast<const uint4*>(src); rr[1] = *reinterpret_cast<const uint4*>(src + 4); }
+        else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<float*>(rr)[u] = src[u];
+      }
+    };
+    uint4 rcur[2], rnext[2];
+    if (p.res.p) load_res(lane, rcur);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < NH; ++h) reg_fence<BN / 2>(acc[h]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);   // the producer refills the stage while this warp runs the epilogue
+    // raw accumulators to the staging rows: row = pixel 16 h + 8 hh + gid, channels 8 j + 2 tig, + 1
+    const uint32_t stg_s = smem_u32(stg);
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          sts64(stg_s + (uint32_t)((16 * h + 8 * hh + gid) * p.stg_ld + (8 * j + 2 * tig) * 4), acc[h][4 * j + 2 * hh], acc[h][4 * j + 2 * hh + 1]);
+    __syncwarp();
+#pragma unroll 1
+    for (int q = lane; q < NPC; q += 32) {
+      if (p.res.p && q + 32 < NPC) load_res(q + 32, rnext);
+      int px, py, c0;
+      if (piece(q, px, py, c0)) {
+        // bias -> act1 -> residual -> act2 -> rounding, element for element as the accumulator pairs had it
+        const uint32_t a = stg_s + (uint32_t)((q / CPP) * p.stg_ld + c0 * 4);
+        const float4 v0 = lds128(a), v1 = lds128(a + 16);
+        float o[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+#pragma unroll
+        for (int u = 0; u < 8; ++u) o[u] += c0 + u < p.cout ? __ldg(p.bias + c0 + u) : 0.f;
+        act_n<8>(o, p.act1, p.slope1, c0, p.cout);
+        if (p.res.p) {
+          if (p.res.f16) {
+#pragma unroll
+            for (int u = 0; u < 8; ++u) o[u] += __half2float(reinterpret_cast<const __half*>(rcur)[u]);
+          } else {
+#pragma unroll
+            for (int u = 0; u < 8; ++u) o[u] += reinterpret_cast<const float*>(rcur)[u];
+          }
+        }
+        if (p.act2 != ACT_NONE) act_n<8>(o, p.act2, p.slope2, c0, p.cout);
+        const bool full = c0 + 8 <= p.cout;
+        const int64_t e = p.out.off(n, py, px) + c0;
+        if (p.out.f16) {
+          __half hv[8];
+#pragma unroll
+          for (int u = 0; u < 8; ++u) hv[u] = __float2half_rn(fminf(fmaxf(o[u], -65504.f), 65504.f));
+          __half* dst = reinterpret_cast<__half*>(p.out.p) + e;
+          if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hv);
+          else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = hv[u];
+        } else {
+          if (p.round_out) {
+#pragma unroll
+            for (int u = 0; u < 8; ++u) o[u] = rn_tf32(o[u]);
+          }
+          float* dst = p.out.p + e;
+          if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+            *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
+            *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
+          } else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = o[u];
+        }
+      }
+      rcur[0] = rnext[0]; rcur[1] = rnext[1];
+    }
+    __syncwarp();   // the staging rows are rewritten by the next tile
   }
 }
 
 }  // namespace tc
 
-template <int BN, bool F16, int NTAPS>
+template <int BN, bool F16, int NTAPS, int RB>
 static void launch_halo(int grid, int smem, gvStream_t stream, const CUtensorMap& a, const CUtensorMap& w, const tc::HaloParams& p) {
   static volatile unsigned char attr[64];   // per (instantiation, device); set once: the layer-dependent size must always fit
-  gv_set_max_smem(tc::conv3x3_halo_kernel<BN, F16, NTAPS>, 227 * 1024, attr);
-  tc::conv3x3_halo_kernel<BN, F16, NTAPS><<<grid, tc::HL_THREADS, smem, stream>>>(a, w, p);
+  gv_set_max_smem(tc::conv3x3_halo_kernel<BN, F16, NTAPS, RB>, 227 * 1024, attr);
+  tc::conv3x3_halo_kernel<BN, F16, NTAPS, RB><<<grid, tc::HL_THREADS, smem, stream>>>(a, w, p);
+}
+
+template <int BN, bool F16, int NTAPS>
+static void launch_halo_rb(bool rb64, int grid, int smem, gvStream_t stream, const CUtensorMap& a, const CUtensorMap& w, const tc::HaloParams& p) {
+  if (rb64) launch_halo<BN, F16, NTAPS, 64>(grid, smem, stream, a, w, p);
+  else launch_halo<BN, F16, NTAPS, 128>(grid, smem, stream, a, w, p);
 }
 
 bool conv2d_halo_supported(const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out) {
@@ -185,31 +271,32 @@ void conv2d_halo(Ctx& cx, const TV& in0, const ConvW& w, const ConvGeom& g, cons
   const int c16 = (w.cout + 15) & ~15;
   const int BN = c16 <= 32 ? 32 : 64;
   if (w.cout_pad < c16) throw std::runtime_error("conv2d_halo: weight padding");
+  const int es = f16 ? 2 : 4;
+  const int rb = in0.c * es <= 64 ? 64 : 128;          // bytes of K per operand row: 32 half / 16 fp32 input channels fit in 64
+  const CUtensorMapSwizzle swz = rb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   CUtensorMap mA, mW;
   {
-    const cuuint64_t es = f16 ? 2 : 4;
     cuuint64_t dims[4] = {(cuuint64_t)in0.c, (cuuint64_t)in0.w, (cuuint64_t)in0.h, (cuuint64_t)in0.n};
     cuuint64_t str[3] = {(cuuint64_t)in0.ld * es, (cuuint64_t)in0.w * in0.ld * es, (cuuint64_t)in0.sn * es};
-    cuuint32_t box[4] = {(cuuint32_t)(f16 ? 64 : 32), (cuuint32_t)HL_TW, (cuuint32_t)(one ? HL_TH : HL_BH), 1};
-    encode(&mA, in0.p, 4, dims, str, box, f16);
+    cuuint32_t box[4] = {(cuuint32_t)(rb / es), (cuuint32_t)HL_TW, (cuuint32_t)(one ? HL_TH : HL_BH), 1};
+    encode(&mA, in0.p, 4, dims, str, box, f16, 1, swz);
   }
-  {   // weights [tap][cout_pad][K block]: rows beyond cout_pad are zero-filled by TMA
+  {   // weights [tap][cout_pad][K block]: rows beyond cout_pad are zero-filled by TMA; a 64-byte box reads the first half of each row
     const int kpad = f16 ? w.cin_pad_h : w.cin_pad;
-    const cuuint64_t es = f16 ? 2 : 4;
     cuuint64_t dims[3] = {(cuuint64_t)kpad, (cuuint64_t)w.cout_pad, (cuuint64_t)ntaps};
     cuuint64_t str[2] = {(cuuint64_t)kpad * es, (cuuint64_t)kpad * w.cout_pad * es};
-    cuuint32_t box[3] = {(cuuint32_t)(f16 ? 64 : 32), (cuuint32_t)BN, (cuuint32_t)ntaps};
-    encode(&mW, f16 ? w.w_tc_h : static_cast<const void*>(w.w_tc), 3, dims, str, box, f16);
+    cuuint32_t box[3] = {(cuuint32_t)(rb / es), (cuuint32_t)BN, (cuuint32_t)ntaps};
+    encode(&mW, f16 ? w.w_tc_h : static_cast<const void*>(w.w_tc), 3, dims, str, box, f16, 1, swz);
   }
   HaloParams p;
   p.tiles_x = (out.w + HL_TW - 1) / HL_TW; p.tiles_y = (out.h + HL_TH - 1) / HL_TH; p.n_img = out.n; p.H = out.h; p.W = out.w; p.cout = w.cout;
   p.origin = (g.loose_w || one) ? 0 : -1; p.round_out = out.f16 ? 0 : 1;
   p.spin_limit = tc_spin_limit();
   p.bias = w.b; p.act1 = e.act1; p.slope1 = e.slope1; p.act2 = e.act2; p.slope2 = e.slope2; p.res = e.res; p.out = out;
-  p.ntaps = ntaps;
-  p.halo_bytes = one ? HL_TW * HL_TH * 128 : 3 * HL_COPY_BYTES;
-  const int w_region = (ntaps * BN * 128 + 1023) & ~1023;
-  const int fixed = w_region + 256 + 1024;
+  p.halo_bytes = (one ? HL_TH : 3 * HL_BH) * HL_TW * rb;
+  p.stg_ld = BN * 4 + 16;
+  const int w_region = (ntaps * BN * rb + 1023) & ~1023;
+  const int fixed = w_region + 8 * (BN == 32 ? 2 : 1) * 16 * p.stg_ld + 256 + 1024;   // (pixels staged per warp: see OWN)
   p.stages = (227 * 1024 - fixed) / p.halo_bytes;
   if (p.stages > HL_MAX_STAGES) p.stages = HL_MAX_STAGES;
   if (p.stages < 2) throw std::runtime_error("conv2d_halo: not enough shared memory");
@@ -223,15 +310,16 @@ void conv2d_halo(Ctx& cx, const TV& in0, const ConvW& w, const ConvGeom& g, cons
     cx.prof->begin(cx.stream, prof_intern(nm), 2.0 * (double)out.n * out.h * out.w * w.cout * (double)w.cin * ntaps);
   }
   const int variant = (BN == 64 ? 4 : 0) | (f16 ? 2 : 0) | (one ? 1 : 0);
+  const bool rb64 = rb == 64;
   switch (variant) {
-    case 0: launch_halo<32, false, 9>(grid, smem, cx.stream, mA, mW, p); break;
-    case 1: launch_halo<32, false, 1>(grid, smem, cx.stream, mA, mW, p); break;
-    case 2: launch_halo<32, true, 9>(grid, smem, cx.stream, mA, mW, p); break;
-    case 3: launch_halo<32, true, 1>(grid, smem, cx.stream, mA, mW, p); break;
-    case 4: launch_halo<64, false, 9>(grid, smem, cx.stream, mA, mW, p); break;
-    case 5: launch_halo<64, false, 1>(grid, smem, cx.stream, mA, mW, p); break;
-    case 6: launch_halo<64, true, 9>(grid, smem, cx.stream, mA, mW, p); break;
-    default: launch_halo<64, true, 1>(grid, smem, cx.stream, mA, mW, p); break;
+    case 0: launch_halo_rb<32, false, 9>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 1: launch_halo_rb<32, false, 1>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 2: launch_halo_rb<32, true, 9>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 3: launch_halo_rb<32, true, 1>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 4: launch_halo_rb<64, false, 9>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 5: launch_halo_rb<64, false, 1>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    case 6: launch_halo_rb<64, true, 9>(rb64, grid, smem, cx.stream, mA, mW, p); break;
+    default: launch_halo_rb<64, true, 1>(rb64, grid, smem, cx.stream, mA, mW, p); break;
   }
   gv_check_launch("conv2d_halo");
   if (cx.prof) cx.prof->end(cx.stream);

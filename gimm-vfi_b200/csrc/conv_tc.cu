@@ -428,10 +428,10 @@ static EncodeTiledFn encode_fn() {
 }
 
 void encode(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
-            bool f16, int pixel_stride) {
+            bool f16, int pixel_stride, CUtensorMapSwizzle swizzle) {
   cuuint32_t estr[5] = {1, (cuuint32_t)pixel_stride, (cuuint32_t)pixel_stride, 1, 1};   // (activation maps: dims 1, 2 = x, y)
   CUresult r = encode_fn()(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("conv_tc: cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
 }

@@ -215,6 +215,7 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t b
   else { static_assert(N == 128, "N"); if constexpr (F16) wgmma_rs_f16_n128(d, a, b, scale_d); else wgmma_rs_tf32_n128(d, a, b, scale_d); }
 }
 
-// host side (defined in conv_tc.cu): cuTensorMapEncodeTiled with SWIZZLE_128B, zero OOB fill; `pixel_stride` = TMA element stride of dims 1, 2
+// host side (defined in conv_tc.cu): cuTensorMapEncodeTiled with zero OOB fill, SWIZZLE_128B unless told otherwise (a 64-byte box row
+// needs SWIZZLE_64B); `pixel_stride` = TMA element stride of dims 1, 2
 void encode(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
-            bool f16 = false, int pixel_stride = 1);
+            bool f16 = false, int pixel_stride = 1, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
