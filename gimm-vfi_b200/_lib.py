@@ -31,6 +31,10 @@ class IO(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in _IO_FIELDS]
 
 
+class Clip(C.Structure):
+    _fields_ = [("frames", C.c_int32), ("pairs", C.c_int32), ("pair_list", C.c_void_p)]
+
+
 class FlowInputs(C.Structure):
     _fields_ = [("flows", C.c_void_p), ("feat4", C.c_void_p * 2), ("feat8", C.c_void_p * 2), ("fnet", C.c_void_p * 2)]
 
@@ -75,6 +79,7 @@ EXPORTS = [
     "gimmvfi_op_alt_corr_forward", "gimmvfi_op_alt_corr_backward",
     "gimmvfi_op_forward_interpolate",
     "gimmvfi_set_motion_config",
+    "gimmvfi_plan_clip", "gimmvfi_forward_clip",
 ]
 
 
@@ -102,6 +107,8 @@ class Lib:
         d.gimmvfi_finalize_weights.argtypes = [vp]
         d.gimmvfi_plan.argtypes = [vp, C.POINTER(Problem), C.POINTER(C.c_size_t)]
         d.gimmvfi_forward.argtypes = [vp, C.POINTER(Problem), C.POINTER(IO), vp, C.c_size_t, vp]
+        d.gimmvfi_plan_clip.argtypes = [vp, C.POINTER(Problem), C.POINTER(Clip), C.POINTER(C.c_size_t)]
+        d.gimmvfi_forward_clip.argtypes = [vp, C.POINTER(Problem), C.POINTER(Clip), C.POINTER(IO), vp, C.c_size_t, vp]
         d.gimmvfi_last_error.argtypes = [vp]
         d.gimmvfi_last_error.restype = C.c_char_p
         d.gimmvfi_last_launches.argtypes = [vp]

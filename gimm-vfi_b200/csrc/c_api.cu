@@ -168,6 +168,31 @@ int gimmvfi_forward(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_i
   GV_TRY(e, { e->eng.forward(to_problem(p), to_io(io), workspace, workspace_bytes, (gvStream_t)cuda_stream); })
 }
 
+static Clip to_clip(const gimmvfi_problem* p, const gimmvfi_clip* c) {
+  if (!p || !c || !c->pair_list) throw std::runtime_error("gimmvfi clip: problem, clip and pair_list are required");
+  if (c->pairs < 1) throw std::runtime_error("gimmvfi clip: at least one pair is required");
+  if (c->frames < 1) throw std::runtime_error("gimmvfi clip: at least one frame is required");
+  if (p->batch != c->pairs) throw std::runtime_error("gimmvfi clip: problem batch must equal the number of pairs");
+  Clip q; q.F = c->frames; q.src.resize(c->pairs); q.tgt.resize(c->pairs);
+  for (int s = 0; s < c->pairs; ++s) {
+    q.src[s] = c->pair_list[2 * s]; q.tgt[s] = c->pair_list[2 * s + 1];
+    if (q.src[s] < 0 || q.src[s] >= q.F || q.tgt[s] < 0 || q.tgt[s] >= q.F)
+      throw std::runtime_error("gimmvfi clip: pair " + std::to_string(s) + " = (" + std::to_string(q.src[s]) + ", " + std::to_string(q.tgt[s]) +
+                               ") indexes outside the " + std::to_string(q.F) + " frames");
+  }
+  return q;
+}
+int gimmvfi_plan_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, size_t* workspace_bytes) {
+  GV_TRY(e, { *workspace_bytes = e->eng.plan_clip(to_problem(p), to_clip(p, clip)); })
+}
+int gimmvfi_forward_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, const gimmvfi_io* io, void* workspace,
+                         size_t workspace_bytes, void* cuda_stream) {
+  GV_TRY(e, {
+    if (!io) throw std::runtime_error("gimmvfi_forward_clip: io is required");
+    e->eng.forward_clip(to_problem(p), to_clip(p, clip), to_io(io), workspace, workspace_bytes, (gvStream_t)cuda_stream);
+  })
+}
+
 int gimmvfi_finalize_weights_synthesis(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_synthesis(); }) }
 int gimmvfi_finalize_weights_f(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_f(); }) }
 int gimmvfi_set_flowformer_iters(gimmvfi_engine* e, int iters) { GV_TRY(e, { if (iters < 1) throw std::runtime_error("iters must be >= 1"); e->eng.ff_iters = iters; }) }

@@ -976,6 +976,38 @@ struct ScaleShiftK {  // y = a*x + b on a dense tensor
   GV_HD void operator()(int64_t i) const { dst[i] = a * src[i] - b; }
 };
 
+// dst sample i <- src sample idx[i]: a clip's per-frame products into pair order.  Whole samples (padding lanes included) as 16- or
+// 4-byte words; the sample list rides in the kernel parameters, kGatherMax samples per launch.
+constexpr int kGatherMax = 64;
+struct alignas(16) Word16 { uint32_t v[4]; };
+template <class Wd> struct GatherSamplesK {
+  const Wd* src; Wd* dst; int64_t words; int idx[kGatherMax];
+  GV_HD void operator()(int64_t i) const {
+    const int64_t n = i / words, k = i - n * words;
+    dst[i] = src[(int64_t)idx[n] * words + k];
+  }
+};
+template <class Wd> static void gather_samples_as(Ctx& cx, const TV& src, const std::vector<int>& idx, const TV& dst, int64_t bytes) {
+  const int64_t words = bytes / (int64_t)sizeof(Wd);
+  for (size_t i0 = 0; i0 < idx.size(); i0 += kGatherMax) {
+    GatherSamplesK<Wd> k{};
+    const int cnt = (int)std::min(idx.size() - i0, (size_t)kGatherMax);
+    for (int i = 0; i < cnt; ++i) k.idx[i] = idx[i0 + i];
+    k.src = reinterpret_cast<const Wd*>(src.p);
+    k.dst = reinterpret_cast<Wd*>(dst.at((int64_t)i0 * dst.sn));
+    k.words = words;
+    parallel_for(cx, (int64_t)cnt * words, k, "clip_gather");
+  }
+}
+static void gather_samples(Ctx& cx, const TV& src, const std::vector<int>& idx, const TV& dst) {
+  if (src.f16 != dst.f16 || src.sn != dst.sn || src.h != dst.h || src.w != dst.w || src.ld != dst.ld || dst.n != (int)idx.size())
+    throw std::runtime_error("clip_gather: source and destination samples differ in shape");
+  for (int i : idx) if (i < 0 || i >= src.n) throw std::runtime_error("clip_gather: sample index out of range");
+  const int64_t bytes = src.sn * (src.f16 ? 2 : 4);
+  if (bytes % 16 == 0 && aligned(src.p, 16) && aligned(dst.p, 16)) gather_samples_as<Word16>(cx, src, idx, dst, bytes);
+  else gather_samples_as<uint32_t>(cx, src, idx, dst, bytes);
+}
+
 static void check_problem(const Problem& p) {
   if (p.B < 1 || p.T < 1) throw std::runtime_error("gimmvfi: B and T must be >= 1");
   const int H = p.H(), W = p.W();
@@ -1033,7 +1065,8 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   // pyramid would not fit the memory budget (a 4K pair without ds_factor: 2 x 78 GB at level 0 alone), NO volume: every lookup
   // computes the 4 x 100 dot products its window needs from the other frame's (pooled, half-precision) features, like
   // BidirCorrBlock's (SURVEY 8(f) row 3, the GPU successor of alt_cuda_corr).  ~5x the time of the volume path, 0 bytes instead of N^2.
-  const double pyr_bytes = (double)S * (double)h * w * (double)h * w * 4.0 * (4.0 / 3.0);
+  // (a clip decides as a batch forward of one pair does - decide_as = 2 directions - so that each of its pairs takes the same path)
+  const double pyr_bytes = (double)(r.decide_as > 0 ? r.decide_as : S) * (double)h * w * (double)h * w * 4.0 * (4.0 / 3.0);
   const bool raft_direct = (raft_direct_ == 1 || (raft_direct_ < 0 && pyr_bytes > raft_direct_auto_bytes_)) && fmap.c == 256 && h >= 16 && w >= 16;
   Pyramid pyr{}; CorrFeat rfeat{};
   if (raft_direct) {
@@ -1150,7 +1183,7 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   tap("raft.net_final", hcur);
 }
 
-void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin) {
+void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin, const Clip* clip) {
   check_problem(P);
   Net N{*this, cx};
   Arena& A = cx.arena;
@@ -1161,41 +1194,65 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   const double inv_d = ds ? (double)Hf / (double)H : 1.0;          // gimmvfi_r.py:297
   const float inv = (float)inv_d, rinv = (float)(1.0 / inv_d);
 
+  // The estimator's pair list over the frame stack: both directions of every pair, [pairs ; reversed pairs], which is also the sample
+  // order of everything downstream.  A batch forward's frames are [I0 batch ; I1 batch]; a clip's are its own F frames, and the
+  // per-frame products they make are gathered into pair order (fslot: a frame's sample among the distinct sources, first-use order).
+  const int NF = clip ? clip->F : 2 * B;
+  std::vector<int> esrc(2 * B), etgt(2 * B), fslot(NF, -1);
+  int nsrc = 0;
+  if (clip) {
+    if (fin) throw std::runtime_error("gimmvfi: a clip runs the engine's own flow estimator");
+    if (clip->F < 1 || (int)clip->src.size() != B || (int)clip->tgt.size() != B) throw std::runtime_error("gimmvfi: bad clip (frames or pair count)");
+    for (int s = 0; s < B; ++s) {
+      if (clip->src[s] < 0 || clip->src[s] >= NF || clip->tgt[s] < 0 || clip->tgt[s] >= NF)
+        throw std::runtime_error("gimmvfi: clip pair " + std::to_string(s) + " indexes outside the " + std::to_string(NF) + " frames");
+      esrc[s] = etgt[B + s] = clip->src[s]; etgt[s] = esrc[B + s] = clip->tgt[s];
+    }
+  } else {
+    for (int s = 0; s < 2 * B; ++s) { esrc[s] = s; etgt[s] = s < B ? s + B : s - B; }
+  }
+  for (int s : esrc) if (fslot[s] < 0) fslot[s] = nsrc++;
+  std::vector<int> pslot(2 * B);   // each sample's distinct-source slot
+  for (int s = 0; s < 2 * B; ++s) pslot[s] = fslot[esrc[s]];
+
   // ------------------------------------------------------------ inputs
-  // frames as NHWC, stacked [I0 batch ; I1 batch]
-  TV full01 = A.tensor(2 * B, Hf, Wf, 3, 4);
-  for (int f = 0; f < 2; ++f)
-    nchw_to_nhwc(cx, io.img_xs + (int64_t)f * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)2 * Hf * Wf, full01.batch(f * B, B), 1.f, 0.f);
+  // frames as NHWC, stacked [I0 batch ; I1 batch] (a clip: its frames in order)
+  TV full01 = A.tensor(NF, Hf, Wf, 3, 4);
+  if (clip)
+    nchw_to_nhwc(cx, io.img_xs, (int64_t)3 * Hf * Wf, (int64_t)Hf * Wf, full01, 1.f, 0.f);
+  else
+    for (int f = 0; f < 2; ++f)
+      nchw_to_nhwc(cx, io.img_xs + (int64_t)f * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)2 * Hf * Wf, full01.batch(f * B, B), 1.f, 0.f);
   TV img01 = full01;
   if (ds) {
-    img01 = A.tensor(2 * B, H, W, 3, 4);
+    img01 = A.tensor(NF, H, W, 3, 4);
     resize_bilinear(cx, full01, img01, rds, rds, 1.f, 0, ACT_NONE);  // gimmvfi_r.py:329-337
   }
-  TV raft_in = A.tensor(2 * B, H, W, 3, 4);
-  TV syn = A.tensor(2 * B, H, W, 3, 4);       // 2*x - 1  (gimmvfi_r.py:230-231)
+  TV raft_in = A.tensor(NF, H, W, 3, 4);
+  TV syn = A.tensor(NF, H, W, 3, 4);       // 2*x - 1  (gimmvfi_r.py:230-231)
   {
     // dense views (ld == 4): run over the padded buffers, padding lane included (harmless)
-    int64_t cnt = (int64_t)2 * B * H * W * 4;
+    int64_t cnt = (int64_t)NF * H * W * 4;
     TV s = img01; s.c = 4; TV d = raft_in; d.c = 4;
     parallel_for(cx, cnt, RaftPrepK{s, d}, "raft_prep");
     parallel_for(cx, cnt, ScaleShiftK{img01.p, syn.p, 2.f, 1.0f}, "img_to_pm1");
   }
   TV synf = syn;
   if (ds) {
-    synf = A.tensor(2 * B, Hf, Wf, 3, 4);
-    parallel_for(cx, (int64_t)2 * B * Hf * Wf * 4, ScaleShiftK{full01.p, synf.p, 2.f, 1.0f}, "img_to_pm1_full");
+    synf = A.tensor(NF, Hf, Wf, 3, 4);
+    parallel_for(cx, (int64_t)NF * Hf * Wf * 4, ScaleShiftK{full01.p, synf.p, 2.f, 1.0f}, "img_to_pm1_full");
   }
 
   // persistent across stages
   TV flow_up = A.tensor(2 * B, H, W, 2);            // [f01 ; f10]
-  TV fmap = A.tensor(2 * B, h, w, 256);             // fnet features of [I0 ; I1]
-  TV feat4 = A.tensor(2 * B, H4, W4, 128), feat8 = A.tensor(2 * B, h, w, 256);  // projected context features
+  TV fmap = A.tensor(NF, h, w, 256);                // fnet features of [I0 ; I1]
+  TV feat4 = A.tensor(nsrc, H4, W4, 128), feat8 = A.tensor(nsrc, h, w, 256);  // projected context features
   float* scaler = A.alloc_f(std::max(B, 64));
 
   // ------------------------------------------------------------ RAFT (both directions batched)
   // The recurrence amplifies operand rounding -> fp32-class arithmetic only: 3xTF32 tensor cores or CUDA cores.
   cx.tc = tc_mode_ >= 2; cx.tc_split = true;
-  TV fproj = A.tensor(2 * B, h, w, 256);            // the maps BidirCorrBlock correlates (R: amt_fproj(fnet map); F: the estimator's own)
+  TV fproj = A.tensor(NF, h, w, 256);               // the maps BidirCorrBlock correlates (R: amt_fproj(fnet map); F: the estimator's own)
   if (fin) {
     // external flow estimator (GIMM-VFI-F): NCHW -> the engine's NHWC buffers, samples [frame-0 batch ; frame-1 batch]
     for (int j = 0; j < 2; ++j) {
@@ -1205,26 +1262,27 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
       nchw_to_nhwc(cx, fin->fnet[j], (int64_t)256 * h * w, (int64_t)h * w, fproj.batch(j * B, B), 1.f, 0.f);
     }
   } else if (is_f()) {
-    // GIMM-VFI-F: the native FlowFormer estimator fills the same four products (gimmvfi_f.py:114-138); F has no feature projections
-    std::vector<int> src(2 * B), tgt(2 * B);   // frames [I0 ; I1]: pairs (b, B + b), then (B + b, b), one reference call per direction
-    for (int s = 0; s < 2 * B; ++s) { src[s] = s; tgt[s] = s < B ? s + B : s - B; }
-    run_flowformer(cx, N, raft_in, src, tgt, B, ff_iters, false, flow_up, TV(), feat4, feat8, fproj);
+    // GIMM-VFI-F: the native FlowFormer estimator fills the same four products (gimmvfi_f.py:114-138); F has no feature projections.
+    // Frames [I0 ; I1]: pairs (b, B + b), then (B + b, b), one reference call per direction; a clip: one reference call per pair and
+    // direction, as a batch forward with B = 1 makes them
+    run_flowformer(cx, N, raft_in, esrc, etgt, clip ? 1 : B, ff_iters, false, flow_up, TV(), feat4, feat8, fproj);
   } else {
     const size_t mk = A.mark();
-    // frame cache (set_frame_cache): with `load` the encoders only see the second frames, samples [B, 2B)
-    const bool fc_on = fc_ != nullptr && !cx.dry;
+    // frame cache (set_frame_cache): with `load` the encoders only see the second frames, samples [B, 2B).  Not for clips.
+    const bool fc_on = fc_ != nullptr && !cx.dry && !clip;
     if (fc_on && fc_bytes_ < frame_cache_bytes(P)) throw std::runtime_error("gimmvfi: frame cache smaller than frame_cache_bytes()");
     const bool fload = fc_on && fc_load_, fstore = fc_on && fc_store_;
     const auto fc_it = fc_valid_.find(fc_);
     if (fload && (fc_it == fc_valid_.end() || fc_it->second.B != B || fc_it->second.H != H || fc_it->second.W != W || fc_it->second.mode != tc_mode_))
       throw std::runtime_error("gimmvfi: frame cache load requested, but this buffer does not hold a frame stored by a forward of the same "
                                "problem size and precision mode");
-    const int e0 = fload ? B : 0, en = fload ? B : 2 * B;
-    // both directions batched: frames [I0 ; I1], pairs (b, B + b) then (B + b, b) (gimmvfi_r.py:126-132)
+    const int e0 = fload ? B : 0, en = fload ? B : nsrc;
+    // both directions batched: frames [I0 ; I1], pairs (b, B + b) then (B + b, b) (gimmvfi_r.py:126-132).  c4 / c8 below are those
+    // of the distinct sources in first-use order, i.e. feat4 / feat8's slots.
     RaftRun r;
     r.img = raft_in; r.iters = raft_iters; r.flow_up = flow_up; r.fmap = fmap; r.enc0 = e0;
-    r.src.resize(2 * B); r.tgt.resize(2 * B);
-    for (int s = 0; s < 2 * B; ++s) { r.src[s] = s; r.tgt[s] = s < B ? s + B : s - B; }
+    r.src = esrc; r.tgt = etgt;
+    if (clip) r.decide_as = 2;   // pair p takes the lookup path of forward() with B = 1 on its frames: the clip's workspace holds 2P volumes
     r.encoded = [&](const TV& c4, const TV& c8, const TV& hx) {
       // context features for the synthesis net (gimmvfi_r.py:134-141)
       N.conv("amt_second_last_cproj", c4, feat4.batch(e0, en));
@@ -1257,6 +1315,19 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   cx.tc = tc_mode_ >= 1; cx.tc_split = false;
   // ------------------------------------------------------------ bidirectional volume on projected features
   if (!fin && !is_f()) N.conv("amt_fproj", fmap, fproj);
+  if (clip) {   // per frame -> pair order: [sources ; targets] of the pairs
+    TV g = A.tensor(2 * B, h, w, 256);
+    gather_samples(cx, fproj, esrc, g);
+    fproj = g;
+    TV s2 = A.tensor(2 * B, H, W, 3, 4);
+    gather_samples(cx, syn, esrc, s2);
+    TV f2 = s2;
+    if (ds) {
+      f2 = A.tensor(2 * B, Hf, Wf, 3, 4);
+      gather_samples(cx, synf, esrc, f2);
+    }
+    syn = s2; synf = f2;
+  }
   // the bidirectional volume only feeds TF32 layers (AMT update blocks) -> plain TF32 is at their input precision
   // Few interpolated frames per pair (T <= corr_direct_max_t): no volume at all - the lookup computes the dot products its window needs
   // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.
@@ -1287,29 +1358,38 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin)
   // ------------------------------------------------------------ hoisted (t-independent) decoder feature upsampling
   TV fup4 = A.tensor(2 * B, H4, W4, 128);   // NewInitDecoder.upsample   fi_components.py:234-244
   TV fup1 = half_chains(cx) ? A.tensor_h(2 * B, H, W, 64) : A.tensor(2 * B, H, W, 64);      // NewMultiFlowDecoder.upsample fi_components.py:284-295
+  // a clip upsamples each distinct source once, then gathers the results into pair order
+  const size_t fup_mk = A.mark();
+  TV fup4s = fup4, fup1s = fup1;
+  if (clip) { fup4s = A.tensor(nsrc, H4, W4, 128); fup1s = half_chains(cx) ? A.tensor_h(nsrc, H, W, 64) : A.tensor(nsrc, H, W, 64); }
   {
     const size_t mk = A.mark();
     const std::string p = "amt_init_decoder.upsample.";
-    TV a = A.tensor(2 * B, H4, W4, 64), b = A.tensor(2 * B, H4, W4, 64), c = A.tensor(2 * B, H4, W4, 128);
+    TV a = A.tensor(nsrc, H4, W4, 64), b = A.tensor(nsrc, H4, W4, 64), c = A.tensor(nsrc, H4, W4, 128);
     pixel_shuffle(cx, feat8, a, 1);
     N.convrelu(p + "1", a, b); N.convrelu(p + "2", b, a); N.convrelu(p + "3", a, b); N.convrelu(p + "4", b, a);
     N.convrelu(p + "5", a, c);
-    N.conv(p + "6", c, fup4, ACT_RELU);  // 1x1 + folded BatchNorm + ReLU
+    N.conv(p + "6", c, fup4s, ACT_RELU);  // 1x1 + folded BatchNorm + ReLU
     A.release(mk);
   }
   {
     const size_t mk = A.mark();
     const std::string p = "amt_final_decoder.upsample.";
     const bool hs = half_chains(cx);
-    TV a = A.tensor(2 * B, H, W, 8);
-    TV b = hs ? A.tensor_h(2 * B, H, W, 32) : A.tensor(2 * B, H, W, 32), c = A.tensor_like(b, 32), d = A.tensor_like(b, 64);
+    TV a = A.tensor(nsrc, H, W, 8);
+    TV b = hs ? A.tensor_h(nsrc, H, W, 32) : A.tensor(nsrc, H, W, 32), c = A.tensor_like(b, 32), d = A.tensor_like(b, 64);
     pixel_shuffle(cx, feat4, a, 2);
     if (cx.tc) N.conv7x(p + "2.0", a, b, ACT_PRELU, N.V(p + "2.1.weight"));   // x-packed 5x5 (pack_xpacked)
     else N.convrelu(p + "2", a, b);
     N.convrelu(p + "3", b, c); N.convrelu(p + "4", c, b); N.convrelu(p + "5", b, c);
     N.convrelu(p + "6", c, d);
-    N.conv(p + "7", d, fup1, ACT_RELU);
+    N.conv(p + "7", d, fup1s, ACT_RELU);
     A.release(mk);
+  }
+  if (clip) {
+    gather_samples(cx, fup4s, pslot, fup4);
+    gather_samples(cx, fup1s, pslot, fup1);
+    if (!debug_) A.release(fup_mk);
   }
   tap("syn.feat4", feat4); tap("syn.feat8", feat8); tap("syn.fup4", fup4); tap("syn.fproj", fproj);
   tap_copy(cx, "syn.fup1", fup1);   // (half in mode 4)
@@ -1749,6 +1829,19 @@ void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t wor
 #endif
     run(cx, p, io);
   });
+}
+
+size_t Engine::plan_clip(const Problem& p, const Clip& c) {
+  need(Entry::Interpolate);
+  const IO io = fake_io();
+  return dry_run([&](Ctx& cx) { run(cx, p, io, nullptr, &c); });
+}
+
+// (eager: a clip's launch sequence depends on its pair list, which the CUDA-graph key of forward() does not hold)
+void Engine::forward_clip(const Problem& p, const Clip& c, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
+  need(Entry::Interpolate);
+  if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: frames, coords, t and imgt_pred are required");
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, nullptr, &c); });
 }
 
 // ---------------------------------------------------------------------------

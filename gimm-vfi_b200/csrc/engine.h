@@ -40,6 +40,13 @@ struct IO {
   float* flowt = nullptr;          // (T,B,2,Hc,Wc)
 };
 
+// A clip (Engine::forward_clip): F frames (IO::img_xs is then (F,3,Hf,Wf)) and Problem::B = P pairs of frame indices, pair p
+// interpolating from frame src[p] to frame tgt[p] at the problem's T timesteps.  Any pairs: reversed, repeated or a frame with itself.
+struct Clip {
+  int F = 0;
+  std::vector<int> src, tgt;
+};
+
 // Outputs of an EXTERNAL bidirectional flow estimator at the network resolution (GIMM-VFI-F: FlowFormer, gimmvfi_f.py:114-138) in the
 // reference's NCHW layouts; with these the engine runs everything downstream of cal_bidirection_flow (forward_from_flow)
 struct FlowInputs {
@@ -90,6 +97,7 @@ struct RaftRun {
   std::vector<int> src, tgt;               // pair s: the flow from frame src[s] to frame tgt[s]
   int iters = 12;
   bool gather = false;                     // always take the gathering path (the planner's upper bound)
+  int decide_as = 0;                       // > 0: choose volume or volume-free lookups as a run of this many pairs would (0: the pair count)
   const float* flow_init = nullptr;        // optional (P,2,H/8,W/8) NCHW, added to coords1 (raft.py:140-141)
   TV flow_up;                              // (P,H,W,2)
   TV flow_low;                             // optional (P,H/8,W/8,2)
@@ -168,6 +176,11 @@ class Engine {
   void forward_lpips(int n, int h, int w, const LpipsIO& io, void* workspace, size_t workspace_bytes, gvStream_t stream);
   size_t plan(const Problem& p);                       // dry run -> workspace bytes
   void forward(const Problem& p, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream);
+  // GIMM-VFI-R / -F over a clip: the per-frame stages (resize, the estimator's encoders, the context projections and the decoders'
+  // feature upsampling) run once per frame, everything after the flow estimate once per pair.  Pair p's outputs are those of forward()
+  // with B = 1 on (frames[src[p]], frames[tgt[p]]).  The plan holds for this clip's pair list.
+  size_t plan_clip(const Problem& p, const Clip& c);
+  void forward_clip(const Problem& p, const Clip& c, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream);
   int64_t last_launches() const { return launches_; }
   // CUDA graphs: forward() records the launch sequence of a (problem, buffers, mode) combination the SECOND time it sees it and
   // replays the instantiated graph afterwards - one cudaGraphLaunch instead of ~550 kernel launches and ~1000 host-side tensor-map
@@ -221,7 +234,7 @@ class Engine {
   void prefix_flow_estimator(std::initializer_list<const char*> children);
   size_t dry_run(const std::function<void(Ctx&)>& run);
   void launch(void* workspace, size_t workspace_bytes, gvStream_t stream, const std::function<void(Ctx&)>& run);
-  void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr);
+  void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr, const Clip* clip = nullptr);
   void finalize_decoders();
   void finalize_flowformer();
   void pack_patch_conv(const std::string& name);

@@ -7,7 +7,7 @@ from typing import Dict, Optional
 
 import torch
 
-from ._lib import IO, FlowInputs, Lib, Problem, View, default_lib
+from ._lib import IO, Clip, FlowInputs, Lib, Problem, View, default_lib
 
 
 # The auxiliary outputs of GIMMVFI_R / GIMMVFI_F.forward: key of the returned dict -> the engine outputs it is made of
@@ -236,13 +236,7 @@ class EngineHandle:
         H, W = (Hf, Wf) if not ds else (int(Hf * ds), int(Wf * ds))
         self._workspace(self.workspace_bytes(B, Hf, Wf, T, ds, Hc, Wc, from_flow=flow_inputs is not None))
         E = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
-        if aux_outputs is None or isinstance(aux_outputs, (bool, int)):
-            aux = _ENGINE_AUX if aux_outputs else ()
-        else:
-            bad = [f for f in aux_outputs if f not in _ENGINE_AUX]
-            if bad:
-                raise ValueError("aux_outputs: unknown engine output(s) %s" % bad)
-            aux = tuple(f for f in _ENGINE_AUX if f in aux_outputs)
+        aux = self._engine_aux(aux_outputs)
         okey = (B, Hf, Wf, T, float(ds) if ds else 0.0, Hc, Wc, aux)
         if self.static_outputs and self._static is not None and self._static[0] == okey:
             out = self._static[1]   # the SAME tensors as the previous call (aliasing is the caller's choice: static_outputs = True)
@@ -254,13 +248,90 @@ class EngineHandle:
             for j in range(2):
                 assert tuple(fi["feat4"][j].shape) == (B, 128, H // 4, W // 4) and tuple(fi["feat8"][j].shape) == (B, 256, H // 8, W // 8)
                 assert tuple(fi["fnet"][j].shape) == (B, 256, H // 8, W // 8)
-        shapes = dict(img_warp_4=(T, B, 3, H, W), flowt0_1=(T, B, 3, 2, Hf, Wf), flowt1_1=(T, B, 3, 2, Hf, Wf),
-                      flowt0_4=(T, B, 2, H // 4, W // 4), flowt1_4=(T, B, 2, H // 4, W // 4), raft_flow=(B, 2, 2, H, W),
-                      nflow=(B, 2, 2, H, W), ninrflow=(T, B, 2, 1, Hc, Wc), flowt=(T, B, 2, Hc, Wc))
+        shapes = self._output_shapes(B, Hf, Wf, T, H, W, Hc, Wc)
         out.update({f: E(*shapes[f]) for f in aux})
         if self.static_outputs:
             self._static = (okey, out)
         return self._launch(out, img_xs, coords, t, B, Hf, Wf, T, ds, Hc, Wc, frame_cache, flow_inputs)
+
+    @staticmethod
+    def _engine_aux(aux_outputs) -> tuple:
+        """forward's aux_outputs -> the engine outputs written besides imgt_pred, in gimmvfi_io order"""
+        if aux_outputs is None or isinstance(aux_outputs, (bool, int)):
+            return _ENGINE_AUX if aux_outputs else ()
+        bad = [f for f in aux_outputs if f not in _ENGINE_AUX]
+        if bad:
+            raise ValueError("aux_outputs: unknown engine output(s) %s" % bad)
+        return tuple(f for f in _ENGINE_AUX if f in aux_outputs)
+
+    @staticmethod
+    def _output_shapes(B, Hf, Wf, T, H, W, Hc, Wc) -> dict:
+        return dict(img_warp_4=(T, B, 3, H, W), flowt0_1=(T, B, 3, 2, Hf, Wf), flowt1_1=(T, B, 3, 2, Hf, Wf),
+                    flowt0_4=(T, B, 2, H // 4, W // 4), flowt1_4=(T, B, 2, H // 4, W // 4), raft_flow=(B, 2, 2, H, W),
+                    nflow=(B, 2, 2, H, W), ninrflow=(T, B, 2, 1, Hc, Wc), flowt=(T, B, 2, Hc, Wc))
+
+    CLIP_PLANS = 16
+
+    @staticmethod
+    def _clip_struct(n_frames: int, pairs):
+        """a gimmvfi_clip and the host pair array it points at (keep both alive for the call)"""
+        pl = [(int(a), int(b)) for a, b in pairs]
+        flat = (C.c_int32 * max(2 * len(pl), 1))(*[i for ab in pl for i in ab])
+        return Clip(int(n_frames), len(pl), C.cast(flat, C.c_void_p)), flat
+
+    def clip_workspace_bytes(self, n_frames, pairs, Hf, Wf, T, ds, Hc, Wc) -> int:
+        """workspace bytes of forward_clip with this frame count and pair list (RAFT's all-pairs volumes grow with the pairs)"""
+        pl = tuple((int(a), int(b)) for a, b in pairs)
+        p = self._problem(len(pl), Hf, Wf, T, ds, Hc, Wc)
+        c, flat = self._clip_struct(n_frames, pl)
+        key = ("clip", int(n_frames), pl, Hf, Wf, T, float(ds) if ds else 0.0, Hc, Wc, self.weights_version)   # (R and F plan differently)
+        if key in self._plans:
+            self._plans[key] = self._plans.pop(key)   # (most recently used last)
+        n = self._plan(key, lambda nb: self.lib.dll.gimmvfi_plan_clip(self._h, C.byref(p), C.byref(c), nb))
+        # the plan depends on the pair list, so the cache keeps only the CLIP_PLANS most recent lists (a video loop reuses one per call size)
+        clip_keys = [k for k in self._plans if k[0] == "clip"]
+        for k in clip_keys[:max(0, len(clip_keys) - self.CLIP_PLANS)]:
+            del self._plans[k]
+        return n
+
+    def forward_clip(self, frames: torch.Tensor, pairs, coords: torch.Tensor, t: torch.Tensor, ds: Optional[float] = None,
+                     aux_outputs=True) -> Dict[str, torch.Tensor]:
+        """A clip in one engine call (gimmvfi_forward_clip): frames (F,3,Hf,Wf) in [0,1], pairs [(src, tgt), ...] of frame indices,
+        coords (T,P,1,Hc,Wc,3), t (T,P), contiguous fp32 on self.device.  Returns forward()'s dict with the pair axis in place of the
+        batch axis: pair p's entries are forward()'s with B = 1 on (frames[src], frames[tgt])."""
+        self._check_inputs(frames, coords, t)
+        if frames.dim() != 4 or frames.shape[1] != 3:
+            raise ValueError("clip: frames must be (F,3,H,W), got %s" % (tuple(frames.shape),))
+        F, _, Hf, Wf = frames.shape
+        pl = [(int(a), int(b)) for a, b in pairs]
+        P = len(pl)
+        if P < 1:
+            raise ValueError("clip: at least one pair is required")
+        bad = [ab for ab in pl if not (0 <= ab[0] < F and 0 <= ab[1] < F)]
+        if bad:
+            raise ValueError("clip: pair(s) %s index outside the %d frames" % (bad, F))
+        if coords.dim() != 6 or coords.shape[1] != P or coords.shape[2] != 1 or coords.shape[5] != 3:
+            raise ValueError("clip: coords must be (T,%d,1,Hc,Wc,3), got %s" % (P, tuple(coords.shape)))
+        T, Hc, Wc = coords.shape[0], coords.shape[3], coords.shape[4]
+        if tuple(t.shape) != (T, P):
+            raise ValueError("clip: t must be (%d,%d), got %s" % (T, P, tuple(t.shape)))
+        H, W = (Hf, Wf) if not ds else (int(Hf * ds), int(Wf * ds))
+        aux = self._engine_aux(aux_outputs)
+        with self._guard():
+            self._workspace(self.clip_workspace_bytes(F, pl, Hf, Wf, T, ds, Hc, Wc))
+            E = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
+            shapes = self._output_shapes(P, Hf, Wf, T, H, W, Hc, Wc)
+            out = {"imgt_pred": E(T, P, 3, Hf, Wf)}
+            out.update({f: E(*shapes[f]) for f in aux})
+            io = IO()
+            io.img_xs, io.coords, io.t = frames.data_ptr(), coords.data_ptr(), t.data_ptr()
+            for k, v in out.items():
+                setattr(io, k, v.data_ptr())
+            p = self._problem(P, Hf, Wf, T, ds, Hc, Wc)
+            c, flat = self._clip_struct(F, pl)
+            self.lib.check(self.lib.dll.gimmvfi_forward_clip(self._h, C.byref(p), C.byref(c), C.byref(io), C.c_void_p(self._ws.data_ptr()),
+                                                             self._ws.numel(), self._stream()), self._h)
+        return out
 
     def _launch(self, out, img_xs, coords, t, B, Hf, Wf, T, ds, Hc, Wc, frame_cache, flow_inputs):
         io = IO()

@@ -117,6 +117,54 @@ class _VFIBase(_GIMMBase):
                         frame_cache=frame_cache if self._raft_encoders else None, flow_inputs=flow_inputs)
         return model_outputs(o, len(t), keys)
 
+    @staticmethod
+    def _check_clip_args(frames, pairs, t):
+        """interpolate's arguments -> (pairs as int tuples, t as floats); raises ValueError before any engine work"""
+        if not torch.is_tensor(frames) or frames.dim() != 4 or frames.shape[1] != 3 or frames.shape[0] < 1:
+            raise ValueError("interpolate: frames must be a (F,3,H,W) tensor with F >= 1, got %s"
+                             % (tuple(frames.shape) if torch.is_tensor(frames) else type(frames).__name__,))
+        F = frames.shape[0]
+        try:
+            pl = [(int(a), int(b)) for a, b in pairs]
+        except (TypeError, ValueError):
+            raise ValueError("interpolate: pairs must be a sequence of (source, target) frame indices")
+        if not pl:
+            raise ValueError("interpolate: the pair list is empty")
+        bad = [ab for ab in pl if not (0 <= ab[0] < F and 0 <= ab[1] < F)]
+        if bad:
+            raise ValueError("interpolate: pair(s) %s index outside the %d frames" % (bad, F))
+        if not isinstance(t, (list, tuple)) or not t:
+            raise ValueError("interpolate: t must be a non-empty list of floats (the timesteps every pair is interpolated at)")
+        try:
+            ts = [float(x) for x in t]
+        except (TypeError, ValueError):
+            raise ValueError("interpolate: t must be a list of floats, one per timestep")
+        return pl, ts
+
+    @torch.no_grad()
+    def interpolate(self, frames, pairs, t, ds_factor=None):
+        """A clip in one engine call: frames (F,3,H,W) in [0,1], pairs [(src, tgt), ...] of frame indices (any: reversed, repeated, a
+        frame with itself), t a list of T floats shared by every pair.  Returns forward()'s dict with the pair axis in place of the batch
+        axis, under the same aux_outputs selection: pair p is forward() on (frames[src], frames[tgt]).  Each frame is resized and encoded
+        once however many pairs use it; the coordinates are sample_coord_input's at the network resolution."""
+        return self._interpolate_clip(frames, pairs, t, ds_factor, self.aux_outputs)
+
+    def _interpolate_clip(self, frames, pairs, t, ds_factor, aux):
+        """interpolate's body; aux: an aux_outputs selection"""
+        pl, ts = self._check_clip_args(frames, pairs, t)
+        if getattr(self, "flow_backend", None) is not None:
+            raise NotImplementedError("interpolate runs the engine's own flow estimator; model.flow_backend is only used by forward()")
+        eng = self._ready(frames)
+        x = frames.to(torch.float32).contiguous()
+        P, (Hf, Wf) = len(pl), x.shape[-2:]
+        ratio = 1.0 if ds_factor is None else ds_factor
+        coords = torch.stack([self.sample_coord_input(P, (Hf, Wf), [ti], device=x.device, upsample_ratio=ratio) for ti in ts], 0)
+        tt = torch.tensor(ts, dtype=torch.float32, device=x.device).unsqueeze(1).expand(len(ts), P).contiguous()
+        keys = aux_keys(aux)
+        o = eng.forward_clip(x, pl, coords.to(torch.float32).contiguous(), tt, ds_factor,
+                             aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]])
+        return model_outputs(o, len(ts), keys)
+
     def compute_psnr(self, preds, targets, reduction="mean"):
         """gimmvfi_r.py:412-426 (the same in gimmvfi_f.py)"""
         assert reduction in ["mean", "sum", "none"]

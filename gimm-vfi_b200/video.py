@@ -93,28 +93,65 @@ class VideoInterpolator:
     RAFT encoder products of each pair's second frame (fnet map, cnet net/inp, projected context features) stay in a device
     cache and are not recomputed when that frame becomes the next pair's first frame (SURVEY.md 8(f) row 2); the outputs
     are bit-identical to independent per-pair calls.  with_flow: push() returns (frames, flow_images) as
-    interpolate_pair_u8(..., with_flow=True) does."""
+    interpolate_pair_u8(..., with_flow=True) does.
 
-    def __init__(self, model, N: int = 2, ds_factor: Optional[float] = None, bgr: bool = True, with_flow: bool = False):
+    pairs_per_call K > 1: push() buffers frames until K pairs are waiting, then interpolates them in one model.interpolate call
+    (K + 1 frames, each encoded once; the last is kept as the next call's first frame) and returns the K (N-1) frames in clip order,
+    pair by pair; the pushes in between return nothing.  flush() interpolates the pairs still waiting at the end of a clip.  With K = 1
+    every push runs its pair at once, through the frame cache above."""
+
+    def __init__(self, model, N: int = 2, ds_factor: Optional[float] = None, bgr: bool = True, with_flow: bool = False,
+                 pairs_per_call: int = 1):
+        if int(pairs_per_call) < 1:
+            raise ValueError("pairs_per_call must be >= 1, got %r" % (pairs_per_call,))
         self.model, self.N, self.ds, self.bgr, self.with_flow = model, int(N), ds_factor, bgr, bool(with_flow)
+        self.pairs_per_call = int(pairs_per_call)
         self._prev = None      # padded float frame (3,H,W) of the last push
         self._padder = None
         self._cache = None     # uint8 device buffer holding the previous frame's encoder products
         self._cache_valid = False
+        self._pending = []     # pairs_per_call > 1: the padded frames pushed after _prev, not yet interpolated
 
     def reset(self):
-        self._prev, self._cache_valid = None, False
+        self._prev, self._cache_valid, self._pending = None, False, []
+
+    def _empty(self):
+        return ([], []) if self.with_flow else []
+
+    @torch.no_grad()
+    def flush(self):
+        """interpolate the pairs still buffered (pairs_per_call > 1) and return their frames as push() does; nothing is left waiting"""
+        if not self._pending:
+            return self._empty()
+        frames = torch.stack([self._prev] + self._pending, 0)            # (k+1,3,H,W)
+        k = len(self._pending)
+        N, aux = self.N, ("flowt",) if self.with_flow else False
+        out = self.model._interpolate_clip(frames, [(i, i + 1) for i in range(k)], [i / N for i in range(1, N)], self.ds, aux)
+        self._prev, self._pending = self._pending[-1], []
+        # out["imgt_pred"][i] is (k,3,H,W): timestep i of every pair -> clip order, pair by pair
+        ims = torch.stack(out["imgt_pred"], 1).reshape(k * (N - 1), *out["imgt_pred"][0].shape[1:])
+        frames_u8 = list(self._padder.unpad_u8(ims, self.bgr).unbind(0)) if N > 1 else []
+        if not self.with_flow:
+            return frames_u8
+        fl = out["flowt"]   # T x (k,2,Hc,Wc), or (2,Hc,Wc) when k == 1 (forward's .squeeze())
+        fl = [f.reshape(k, *f.shape[-3:]) for f in fl]
+        return frames_u8, flow_images(self._padder, [fl[i][p] for p in range(k) for i in range(N - 1)], self.bgr)
 
     @torch.no_grad()
     def push(self, frame_u8: torch.Tensor):
         dev = frame_u8.device
         if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
+            if self._pending:
+                raise ValueError("VideoInterpolator: the frame size changed with pairs still buffered; flush() first")
             self._padder = InputPadder(frame_u8.shape[:2], 32)
             self.reset()
         cur = self._padder.pad_u8(frame_u8.unsqueeze(0))[0]              # (3,H,W)
         if self._prev is None:
             self._prev = cur
-            return ([], []) if self.with_flow else []
+            return self._empty()
+        if self.pairs_per_call > 1:
+            self._pending.append(cur)
+            return self.flush() if len(self._pending) == self.pairs_per_call else self._empty()
         m = self.model
         xs = torch.stack([self._prev, cur], 1).unsqueeze(0).contiguous()  # (1,3,2,H,W)
         H, W = xs.shape[-2:]

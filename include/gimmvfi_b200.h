@@ -78,6 +78,27 @@ int gimmvfi_finalize_weights(gimmvfi_engine* e);
 int gimmvfi_plan(gimmvfi_engine* e, const gimmvfi_problem* p, size_t* workspace_bytes);
 int gimmvfi_forward(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_io* io, void* workspace, size_t workspace_bytes,
                     void* cuda_stream);
+/* ---- A clip in one call (GIMM-VFI-R and GIMM-VFI-F with their own estimator) ----
+ * `frames` frames and `pairs` (source, target) pairs of frame indices, every pair interpolated at the same T timesteps.  Any pairs are
+ * allowed: consecutive or not, reversed, repeated, or a frame with itself.  Per frame: the ds_factor resize, the estimator's encoders
+ * (RAFT fnet / cnet, FlowFormer's Twins), the context projections and the decoders' feature upsampling; per pair: correlation, the
+ * estimator's iterations, GIMM and the synthesis.  Pair p's outputs are gimmvfi_forward's with batch 1 on (frame src, frame tgt): the
+ * same estimator path (RAFT chooses its volume or volume-free lookup as for one pair) and flows, and the splat's float-atomic
+ * summation order as the only difference behind it.
+ * problem->batch must equal pairs; io->img_xs points at the frames, (F,3,Hf,Wf) in [0,1]; coords (T,P,1,Hc,Wc,3), t (T,P); the
+ * outputs are gimmvfi_io's with P in place of B.  The workspace holds P pairs' correlation volumes (RAFT's all-pairs pyramid grows
+ * with P): gimmvfi_plan_clip reports it for this pair list, to choose how many pairs one call takes.  A pair list whose volumes do
+ * not fit the device needs fewer pairs per call; the clip never changes a pair's lookup path to make them fit.  Not recorded as a
+ * CUDA graph; the frame cache does not apply. */
+typedef struct gimmvfi_clip {
+  int32_t frames;              /* F >= 1                                      */
+  int32_t pairs;               /* P >= 1                                      */
+  const int32_t* pair_list;    /* HOST (P,2): source, target frame index     */
+} gimmvfi_clip;
+int gimmvfi_plan_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, size_t* workspace_bytes);
+int gimmvfi_forward_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, const gimmvfi_io* io, void* workspace,
+                         size_t workspace_bytes, void* cuda_stream);
+
 /* ---- GIMM-VFI-F (gimmvfi_f.py): everything downstream of the flow estimator ----
  * GIMMVFI_F.forward = FlowFormer (cal_bidirection_flow, gimmvfi_f.py:114-138) + exactly the GIMM / synthesis stages of GIMM-VFI-R
  * without the feature projections.  Those stages run natively on the outputs of an EXTERNAL estimator, given in the reference's

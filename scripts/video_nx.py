@@ -36,6 +36,8 @@ def parse_args(argv=None):
     p.add_argument("--N", type=int, default=8)
     p.add_argument("--ds-factor", type=float, default=1.0)
     p.add_argument("--frames", action="store_true", help="write PNG sequences output/%%04d.png and flow/%%04d.png instead of videos")
+    p.add_argument("--pairs-per-call", type=int, default=1,
+                   help="interpolate K consecutive pairs per engine call, each frame encoded once (1: one call per pair)")
     return p.parse_args(argv)
 
 
@@ -99,21 +101,34 @@ def main(argv=None):
     out = FrameSink(os.path.join(args.output_path, "output.mp4"), os.path.join(args.output_path, "output"), fps, args.frames)
     flow = FrameSink(os.path.join(args.output_path, "flow.mp4"), os.path.join(args.output_path, "flow"), fps, args.frames)
     ds = None if args.ds_factor == 1.0 else args.ds_factor   # a resize by 1 is the identity
-    vi = VideoInterpolator(model, N=args.N, ds_factor=ds, bgr=True, with_flow=True)
+    vi = VideoInterpolator(model, N=args.N, ds_factor=ds, bgr=True, with_flow=True, pairs_per_call=args.pairs_per_call)
     host = lambda x: x.cpu().numpy()
-    prev_bgr = None
+    waiting = []   # originals whose interpolated frames have not come back yet (pairs_per_call > 1), oldest first
+    per_pair = args.N - 1
+
+    def emit(frames, flows, last):
+        # frames / flows: N-1 per pair, in clip order; the pair from waiting[k] to waiting[k + 1]
+        for k in range(len(frames) // per_pair if per_pair else 0):
+            prev = waiting.pop(0)
+            for fr, fl in zip(frames[k * per_pair:(k + 1) * per_pair], flows[k * per_pair:(k + 1) * per_pair]):
+                out.write(host(torch.cat([prev, fr], 1)))
+                flow.write(host(fl))
+            if len(waiting) > 1 or not last:   # the reference appends every original twice-wide and drops the last image
+                out.write(host(torch.cat([waiting[0], waiting[0]], 1)))
+
     for j, name in enumerate(names):
         bgr = cv2.imread(os.path.join(args.source_path, name), cv2.IMREAD_COLOR)
         if bgr is None:
             raise SystemExit("video_nx.py: cannot read %s" % name)
         cur_bgr = torch.from_numpy(bgr).to(dev)
-        frames, flows = vi.push(cur_bgr.flip(-1).contiguous())   # RGB in; frames come back BGR
-        for fr, fl in zip(frames, flows):
-            out.write(host(torch.cat([prev_bgr, fr], 1)))
-            flow.write(host(fl))
-        if j < len(names) - 1:   # the reference appends every original twice-wide and drops the last image
+        last = j == len(names) - 1
+        if j == 0 and not last:   # (the reference drops the last image: a one-image input writes nothing)
             out.write(host(torch.cat([cur_bgr, cur_bgr], 1)))
-        prev_bgr = cur_bgr
+        waiting.append(cur_bgr)
+        frames, flows = vi.push(cur_bgr.flip(-1).contiguous())   # RGB in; frames come back BGR
+        emit(frames, flows, last)
+        if last:
+            emit(*vi.flush(), last)
         print("frame %d / %d" % (j + 1, len(names)), flush=True)
     out.close()
     flow.close()
