@@ -70,7 +70,7 @@ EXPORTS = [
     "gimmvfi_get_tap", "gimmvfi_build_info", "gimmvfi_set_profile", "gimmvfi_profile_json",
     "gimmvfi_set_tensor_cores", "gimmvfi_set_cuda_graph", "gimmvfi_graph_replays", "gimmvfi_finalize_weights_gimm", "gimmvfi_finalize_weights_synthesis", "gimmvfi_finalize_weights_f", "gimmvfi_set_flowformer_iters", "gimmvfi_plan_from_flow", "gimmvfi_forward_from_flow", "gimmvfi_gimm_plan", "gimmvfi_gimm_forward", "gimmvfi_frame_cache_bytes", "gimmvfi_set_frame_cache", "gimmvfi_op_conv2d_tc", "gimmvfi_op_conv2d_tc_f16", "gimmvfi_op_conv2d_tc_strided", "gimmvfi_op_frames_u8_to_padded_f32", "gimmvfi_op_pred_to_u8", "gimmvfi_op_softsplat", "gimmvfi_op_softsplat_fused", "gimmvfi_op_backwarp", "gimmvfi_op_layernorm", "gimmvfi_op_window_attention", "gimmvfi_op_global_attention", "gimmvfi_op_patchify", "gimmvfi_op_cost_conv1", "gimmvfi_op_conv7x7_small_cout", "gimmvfi_op_row_softmax", "gimmvfi_op_resize",
     "gimmvfi_op_corr_volume", "gimmvfi_op_corr_volume_tc", "gimmvfi_op_corr_pool", "gimmvfi_op_corr_pool_pyramid", "gimmvfi_op_corr_lookup", "gimmvfi_op_corr_lookup_direct", "gimmvfi_op_conv2d",
-    "gimmvfi_instnorm_scratch_floats", "gimmvfi_op_hyponet", "gimmvfi_op_conv2d_halo", "gimmvfi_op_instnorm", "gimmvfi_op_convex_upsample", "gimmvfi_op_pixel_shuffle", "gimmvfi_op_tail_pointwise",
+    "gimmvfi_instnorm_scratch_floats", "gimmvfi_op_hyponet", "gimmvfi_op_conv2d_halo", "gimmvfi_op_conv2d_wide", "gimmvfi_op_instnorm", "gimmvfi_op_convex_upsample", "gimmvfi_op_pixel_shuffle", "gimmvfi_op_tail_pointwise",
     "gimmvfi_flow_to_image_scratch_floats", "gimmvfi_op_flow_to_image",
     "gimmvfi_finalize_weights_lpips", "gimmvfi_lpips_plan", "gimmvfi_lpips_forward",
     "gimmvfi_finalize_weights_flowformer", "gimmvfi_flowformer_plan", "gimmvfi_flowformer_forward", "gimmvfi_flowformer_forward_ex",

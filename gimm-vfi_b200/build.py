@@ -6,7 +6,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["ops_pointwise.cu", "corr.cu", "conv.cu", "conv_tc.cu", "conv_halo.cu", "corr_gemm.cu", "hyponet.cu", "ops_tokens.cu", "flowformer.cu", "engine.cu", "c_api.cu"]
+SOURCES = ["ops_pointwise.cu", "corr.cu", "conv.cu", "conv_tc.cu", "conv_halo.cu", "conv_wide.cu", "corr_gemm.cu", "hyponet.cu", "ops_tokens.cu", "flowformer.cu", "engine.cu", "c_api.cu"]
 OUT = os.path.join(HERE, "libgimmvfi_b200.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-diag-suppress", "550"]

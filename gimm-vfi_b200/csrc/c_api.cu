@@ -606,6 +606,27 @@ int gimmvfi_op_conv2d_tc_f16(const gimmvfi_view* in0, const gimmvfi_view* in1, c
 #endif
   })
 }
+int gimmvfi_op_conv2d_wide(const gimmvfi_view* in0, const gimmvfi_view* in1, const void* w_tc_h, const float* bias, int cin, int cout,
+                           int act1, const float* slope1, const gimmvfi_view* residual, int act2, const float* slope2, int half_mask,
+                           const gimmvfi_view* out, void* stream) {
+  gimmvfi_engine* e = nullptr;
+  GV_TRY(e, {
+#ifdef GV_HOSTSIM
+    throw std::runtime_error("conv2d_wide is a tensor-core kernel; not available in the host simulation");
+#else
+    Ctx cx = op_ctx(stream);
+    ConvW w; w.b = bias; w.cin = cin; w.cout = cout; w.kh = 3; w.kw = 3;
+    w.cout_pad = tc_cout_pad(cout); w.w_tc_h = w_tc_h; w.cin_pad_h = (cin + 63) & ~63;
+    ConvGeom g; g.stride = 1; g.ph = 1; g.pw = 1;
+    TV a0 = to_tv(in0); TV a1 = to_tv(in1); TV r = to_tv(residual); TV o = to_tv(out);
+    a0.f16 = half_mask & 1; if (a1.p) a1.f16 = half_mask & 1; o.f16 = (half_mask >> 1) & 1; if (r.p) r.f16 = (half_mask >> 2) & 1;
+    ConvEpi ep; ep.act1 = act1; ep.slope1 = slope1; ep.res = r; ep.act2 = act2; ep.slope2 = slope2;
+    if (a0.c + (a1.p ? a1.c : 0) != cin || o.c != cout) throw std::runtime_error("conv2d_wide: channel counts do not match the views");
+    if (!conv2d_wide_supported(a0, a1, w, g, ep, o)) throw std::runtime_error("conv2d_wide: unsupported configuration");
+    conv2d_wide(cx, a0, a1, w, g, ep, o);
+#endif
+  })
+}
 int gimmvfi_op_conv2d_halo(const gimmvfi_view* in0, const void* w_tc_h, const float* w_tc, const float* bias, int cin, int cout, int act1,
                            const float* slope1, const gimmvfi_view* residual, int act2, const float* slope2, int half_mask, int prepadded,
                            const gimmvfi_view* out, void* stream) {

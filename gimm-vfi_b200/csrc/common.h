@@ -391,6 +391,10 @@ void corr_gemm_3xf16(Ctx& cx, const void* a_planes, int64_t a_plane, int M, cons
 // tile + halo loaded once (three x-shifted copies) and every tap an MMA on a 1024-byte aligned view of it, weights resident
 bool conv2d_halo_supported(const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out);
 void conv2d_halo(Ctx& cx, const TV& in0, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out);
+// conv_wide.cu (sm_90a): 3x3 stride-1 convolutions of wide half layers (input segments of whole 64-channel blocks, cout a multiple of
+// 128: the final decoder's 256-channel trunk) with each K block's activation tile + halo loaded once and the weights streamed per tap
+bool conv2d_wide_supported(const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out);
+void conv2d_wide(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const ConvGeom& g, const ConvEpi& e, const TV& out);
 // hyponet.cu (sm_90a; the host simulation emulates its arithmetic): the whole HypoNet MLP in one kernel
 bool hyponet_fused_supported(const TV& lat, const TV& out);
 void hyponet_fused(Ctx& cx, const TV& lat /*n,h,w,32*/, const float* coords /*n*h*w x (t,y,x)*/, const void* blob /*hypo:: layout*/, const TV& out /*2 ch*/);

@@ -493,6 +493,11 @@ void conv2d(Ctx& cx, const TV& in0, const TV& in1, const ConvW& w, const ConvGeo
     conv2d_halo(cx, in0, w, g, e, out);
     return;
   }
+  // wide half 3x3 layers (the final decoder trunk): each K block's tile + halo loaded once, the nine taps as views of it
+  if (cx.tc && conv2d_wide_supported(in0, in1, w, g, e, out)) {
+    conv2d_wide(cx, in0, in1, w, g, e, out);
+    return;
+  }
 #endif
   if (cx.tc && conv2d_tc_supported(in0, in1, w, g, e, out, cx.tc_split && !any_f16)) { conv2d_tc(cx, in0, in1, w, g, e, out, cx.tc_split && !any_f16); return; }
   if (any_f16) throw std::runtime_error("conv2d: half-precision tensors are only handled by the tensor-core path (layer not eligible)");

@@ -142,10 +142,8 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
       }
     }
     wgmma_commit();
-    // The epilogue works on 8-channel pieces of whole pixels: the warp's NH x 16 pixels (image rows 8 h + 2 wq, + 1 with OWN, else
-    // 8 wg + 2 wq, + 1; columns 0-7) x BN channels.  A runtime loop over the pieces keeps ONE copy of the activation code: unrolled
-    // over the accumulator pairs it was ~5k instructions per kernel, the epilogue bound by instruction fetch.  The residual of the
-    // lane's next piece is read before the current piece is computed, the first one while the MMAs run.
+    // The epilogue works on 8-channel pieces of whole pixels (epi_pieces): the warp's NH x 16 pixels (image rows 8 h + 2 wq, + 1 with
+    // OWN, else 8 wg + 2 wq, + 1; columns 0-7) x BN channels.  The first piece's residual is read while the MMAs run.
     constexpr int CPP = BN / 8;            // pieces per pixel
     constexpr int NPC = NH * 16 * CPP;     // pieces per warp and tile (a multiple of 32)
     const int yw = ty * HL_TH + (OWN ? 0 : 8 * wg) + wq * 2;
@@ -154,24 +152,8 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
       px = tx * HL_TW + (pix & 7); py = yw + 8 * (pix >> 4) + ((pix >> 3) & 1); c0 = (q % CPP) * 8;
       return px < p.W && py < p.H && c0 < p.cout;
     };
-    // the residual of piece q as raw storage bits (8 halves in r[0], or 8 floats in r[0], r[1])
-    auto load_res = [&](int q, uint4* rr) {
-      int px, py, c0;
-      rr[0] = rr[1] = make_uint4(0u, 0u, 0u, 0u);
-      if (!piece(q, px, py, c0)) return;
-      const int64_t e = p.res.off(n, py, px) + c0;
-      if (p.res.f16) {
-        const __half* src = reinterpret_cast<const __half*>(p.res.p) + e;
-        if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) rr[0] = *reinterpret_cast<const uint4*>(src);
-        else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<__half*>(rr)[u] = src[u];
-      } else {
-        const float* src = p.res.p + e;
-        if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) { rr[0] = *reinterpret_cast<const uint4*>(src); rr[1] = *reinterpret_cast<const uint4*>(src + 4); }
-        else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<float*>(rr)[u] = src[u];
-      }
-    };
-    uint4 rcur[2], rnext[2];
-    if (p.res.p) load_res(lane, rcur);
+    uint4 rcur[2];
+    if (p.res.p) epi_load_res(p, n, lane, piece, rcur);
     wgmma_wait<0>();
 #pragma unroll
     for (int h = 0; h < NH; ++h) reg_fence<BN / 2>(acc[h]);
@@ -187,51 +169,7 @@ __global__ void __launch_bounds__(HL_THREADS, 1) conv3x3_halo_kernel(const __gri
         for (int hh = 0; hh < 2; ++hh)
           sts64(stg_s + (uint32_t)((16 * h + 8 * hh + gid) * p.stg_ld + (8 * j + 2 * tig) * 4), acc[h][4 * j + 2 * hh], acc[h][4 * j + 2 * hh + 1]);
     __syncwarp();
-#pragma unroll 1
-    for (int q = lane; q < NPC; q += 32) {
-      if (p.res.p && q + 32 < NPC) load_res(q + 32, rnext);
-      int px, py, c0;
-      if (piece(q, px, py, c0)) {
-        // bias -> act1 -> residual -> act2 -> rounding, element for element as the accumulator pairs had it
-        const uint32_t a = stg_s + (uint32_t)((q / CPP) * p.stg_ld + c0 * 4);
-        const float4 v0 = lds128(a), v1 = lds128(a + 16);
-        float o[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-#pragma unroll
-        for (int u = 0; u < 8; ++u) o[u] += c0 + u < p.cout ? __ldg(p.bias + c0 + u) : 0.f;
-        act_n<8>(o, p.act1, p.slope1, c0, p.cout);
-        if (p.res.p) {
-          if (p.res.f16) {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) o[u] += __half2float(reinterpret_cast<const __half*>(rcur)[u]);
-          } else {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) o[u] += reinterpret_cast<const float*>(rcur)[u];
-          }
-        }
-        if (p.act2 != ACT_NONE) act_n<8>(o, p.act2, p.slope2, c0, p.cout);
-        const bool full = c0 + 8 <= p.cout;
-        const int64_t e = p.out.off(n, py, px) + c0;
-        if (p.out.f16) {
-          __half hv[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) hv[u] = __float2half_rn(fminf(fmaxf(o[u], -65504.f), 65504.f));
-          __half* dst = reinterpret_cast<__half*>(p.out.p) + e;
-          if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hv);
-          else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = hv[u];
-        } else {
-          if (p.round_out) {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) o[u] = rn_tf32(o[u]);
-          }
-          float* dst = p.out.p + e;
-          if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-            *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
-            *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
-          } else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = o[u];
-        }
-      }
-      rcur[0] = rnext[0]; rcur[1] = rnext[1];
-    }
+    epi_pieces<NPC, CPP>(p, n, stg_s, p.stg_ld, lane, piece, rcur);
     __syncwarp();   // the staging rows are rewritten by the next tile
   }
 }

@@ -1,4 +1,4 @@
-// Epilogue building blocks of the tensor-core convolutions (conv_tc.cu, conv_halo.cu): activations, 4-channel loads / stores of
+// Epilogue building blocks of the tensor-core convolutions (conv_tc.cu, conv_halo.cu, conv_wide.cu): activations, 4-channel loads / stores of
 // fp32 or half tensors, shared-memory 128-bit accessors.  Device code only; include inside namespace gv::tc after tc_ptx.cuh.
 #pragma once
 
@@ -146,5 +146,81 @@ __device__ __forceinline__ void act_rows(float* o, int act, const float* slope, 
       for (int u = 0; u < 4; ++u) o[4 * r + u] = o[4 * r + u] > 0.f ? o[4 * r + u] : sl[u] * o[4 * r + u];
   } else {
     act_n<4 * R>(o, act, slope, c, cout);   // (channel-independent activations)
+  }
+}
+
+// ---- the per-pixel epilogue of conv_halo.cu and conv_wide.cu: one warp's raw accumulators are staged in shared memory as pixel rows
+// of stg_ld bytes (8-channel piece k of staged pixel i at i * stg_ld + 32 k), and a loop over 8-channel pieces of whole pixels applies
+// bias -> act1 -> residual -> act2 -> rounding and stores 16 or 32 bytes of the NHWC output.  A runtime loop keeps ONE copy of the
+// activation code (unrolled over accumulator pairs it was ~5k instructions, instruction-fetch bound).  P has the fields H, W, cout,
+// round_out, bias, act1, slope1, act2, slope2, res, out; piece(q, px, py, c0) maps piece q (staged pixel q / CPP, piece q % CPP) to
+// its output pixel and first channel and tells whether it is inside the output.
+
+// the residual of piece q as raw storage bits (8 halves in r[0], or 8 floats in r[0], r[1])
+template <class P, class Piece>
+__device__ __forceinline__ void epi_load_res(const P& p, int n, int q, const Piece& piece, uint4* rr) {
+  int px, py, c0;
+  rr[0] = rr[1] = make_uint4(0u, 0u, 0u, 0u);
+  if (!piece(q, px, py, c0)) return;
+  const int64_t e = p.res.off(n, py, px) + c0;
+  if (p.res.f16) {
+    const __half* src = reinterpret_cast<const __half*>(p.res.p) + e;
+    if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) rr[0] = *reinterpret_cast<const uint4*>(src);
+    else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<__half*>(rr)[u] = src[u];
+  } else {
+    const float* src = p.res.p + e;
+    if (c0 + 8 <= p.cout && (reinterpret_cast<uintptr_t>(src) & 15) == 0) { rr[0] = *reinterpret_cast<const uint4*>(src); rr[1] = *reinterpret_cast<const uint4*>(src + 4); }
+    else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) reinterpret_cast<float*>(rr)[u] = src[u];
+  }
+}
+
+// pieces lane, lane + 32, ... < NPC; rcur holds the residual of piece `lane` (epi_load_res, issued early by the caller: e.g. while
+// the MMAs run); each piece's successor's residual is read before the piece is computed
+template <int NPC, int CPP, class P, class Piece>
+__device__ __forceinline__ void epi_pieces(const P& p, int n, uint32_t stg_s, int stg_ld, int lane, const Piece& piece, uint4* rcur) {
+  uint4 rnext[2];
+#pragma unroll 1
+  for (int q = lane; q < NPC; q += 32) {
+    if (p.res.p && q + 32 < NPC) epi_load_res(p, n, q + 32, piece, rnext);
+    int px, py, c0;
+    if (piece(q, px, py, c0)) {
+      const uint32_t a = stg_s + (uint32_t)((q / CPP) * stg_ld + (q % CPP) * 32);
+      const float4 v0 = lds128(a), v1 = lds128(a + 16);
+      float o[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+#pragma unroll
+      for (int u = 0; u < 8; ++u) o[u] += c0 + u < p.cout ? __ldg(p.bias + c0 + u) : 0.f;
+      act_n<8>(o, p.act1, p.slope1, c0, p.cout);
+      if (p.res.p) {
+        if (p.res.f16) {
+#pragma unroll
+          for (int u = 0; u < 8; ++u) o[u] += __half2float(reinterpret_cast<const __half*>(rcur)[u]);
+        } else {
+#pragma unroll
+          for (int u = 0; u < 8; ++u) o[u] += reinterpret_cast<const float*>(rcur)[u];
+        }
+      }
+      if (p.act2 != ACT_NONE) act_n<8>(o, p.act2, p.slope2, c0, p.cout);
+      const bool full = c0 + 8 <= p.cout;
+      const int64_t e = p.out.off(n, py, px) + c0;
+      if (p.out.f16) {
+        __half hv[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) hv[u] = __float2half_rn(fminf(fmaxf(o[u], -65504.f), 65504.f));
+        __half* dst = reinterpret_cast<__half*>(p.out.p) + e;
+        if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hv);
+        else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = hv[u];
+      } else {
+        if (p.round_out) {
+#pragma unroll
+          for (int u = 0; u < 8; ++u) o[u] = rn_tf32(o[u]);
+        }
+        float* dst = p.out.p + e;
+        if (full && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+          *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
+          *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
+        } else for (int u = 0; u < 8 && c0 + u < p.cout; ++u) dst[u] = o[u];
+      }
+    }
+    rcur[0] = rnext[0]; rcur[1] = rnext[1];
   }
 }

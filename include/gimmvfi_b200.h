@@ -388,6 +388,14 @@ int gimmvfi_op_conv2d_tc_f16(const gimmvfi_view* in0, const gimmvfi_view* in1_or
                              const float* bias, int cin, int cout, int kh, int kw, int act1, const float* slope1,
                              const gimmvfi_view* residual_or_null, int act2, const float* slope2, int half_mask,
                              const gimmvfi_view* out, void* stream);
+/* 3x3 stride-1 convolution with zero padding 1 of a wide half layer (csrc/conv_wide.cu: the final decoder's 256-channel trunk): each
+ * 64-channel K block's tile + halo is loaded once and the nine taps are MMAs on views of it.  in0 (and in1) hold IEEE half and have
+ * channels that are multiples of 64 (16-byte aligned views), cin = their sum, cout a multiple of 128; w_tc_h and the epilogue as
+ * gimmvfi_op_conv2d_tc_f16 (half_mask bit 0 must be set; bit 1 = out is half, bit 2 = residual is half).  The residual may be the
+ * output itself (in-place ResBlock tail). */
+int gimmvfi_op_conv2d_wide(const gimmvfi_view* in0, const gimmvfi_view* in1_or_null, const void* w_tc_h, const float* bias, int cin, int cout,
+                           int act1, const float* slope1, const gimmvfi_view* residual_or_null, int act2, const float* slope2, int half_mask,
+                           const gimmvfi_view* out, void* stream);
 /* nn.InstanceNorm2d + optional relu: raft/extractor.py:133-134; scratch >= gimmvfi_instnorm_scratch_floats */
 /* 3x3 (or 1x1) stride-1 convolution of a K-poor layer (cin <= 32 fp32 or <= 64 half, cout <= 64): tile + halo loaded once, the taps as
  * MMAs on views of it, weights resident in shared memory (csrc/conv_halo.cu).  Weight packing as gimmvfi_op_conv2d_tc (plane 0) /
