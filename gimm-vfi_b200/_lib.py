@@ -35,6 +35,10 @@ class Clip(C.Structure):
     _fields_ = [("frames", C.c_int32), ("pairs", C.c_int32), ("pair_list", C.c_void_p)]
 
 
+class Queries(C.Structure):
+    _fields_ = [("frames", C.c_int32), ("queries", C.c_int32), ("pair_list", C.c_void_p), ("t", C.c_void_p)]
+
+
 class FlowInputs(C.Structure):
     _fields_ = [("flows", C.c_void_p), ("feat4", C.c_void_p * 2), ("feat8", C.c_void_p * 2), ("fnet", C.c_void_p * 2)]
 
@@ -80,6 +84,7 @@ EXPORTS = [
     "gimmvfi_op_forward_interpolate",
     "gimmvfi_set_motion_config",
     "gimmvfi_plan_clip", "gimmvfi_forward_clip",
+    "gimmvfi_plan_queries", "gimmvfi_forward_queries", "gimmvfi_set_coord_range",
 ]
 
 
@@ -109,6 +114,9 @@ class Lib:
         d.gimmvfi_forward.argtypes = [vp, C.POINTER(Problem), C.POINTER(IO), vp, C.c_size_t, vp]
         d.gimmvfi_plan_clip.argtypes = [vp, C.POINTER(Problem), C.POINTER(Clip), C.POINTER(C.c_size_t)]
         d.gimmvfi_forward_clip.argtypes = [vp, C.POINTER(Problem), C.POINTER(Clip), C.POINTER(IO), vp, C.c_size_t, vp]
+        d.gimmvfi_plan_queries.argtypes = [vp, C.POINTER(Problem), C.POINTER(Queries), C.POINTER(C.c_size_t)]
+        d.gimmvfi_forward_queries.argtypes = [vp, C.POINTER(Problem), C.POINTER(Queries), C.POINTER(IO), vp, C.c_size_t, vp]
+        d.gimmvfi_set_coord_range.argtypes = [vp, C.c_double, C.c_double]
         d.gimmvfi_last_error.argtypes = [vp]
         d.gimmvfi_last_error.restype = C.c_char_p
         d.gimmvfi_last_launches.argtypes = [vp]

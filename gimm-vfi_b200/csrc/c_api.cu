@@ -193,6 +193,31 @@ int gimmvfi_forward_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimm
   })
 }
 
+static Queries to_queries(const gimmvfi_problem* p, const gimmvfi_queries* q) {
+  if (!p || !q || !q->pair_list || !q->t) throw std::runtime_error("gimmvfi queries: problem, queries, pair_list and t are required");
+  if (q->queries < 1) throw std::runtime_error("gimmvfi queries: at least one query is required");
+  if (q->frames < 1) throw std::runtime_error("gimmvfi queries: at least one frame is required");
+  Queries r; r.F = q->frames;
+  for (int i = 0; i < q->queries; ++i) { r.src.push_back(q->pair_list[2 * i]); r.tgt.push_back(q->pair_list[2 * i + 1]); r.t.push_back(q->t[i]); }
+  return r;   // (indices and t are checked by the engine's schedule)
+}
+int gimmvfi_plan_queries(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_queries* queries, size_t* workspace_bytes) {
+  GV_TRY(e, { *workspace_bytes = e->eng.plan_queries(to_problem(p), to_queries(p, queries)); })
+}
+int gimmvfi_forward_queries(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_queries* queries, const gimmvfi_io* io, void* workspace,
+                            size_t workspace_bytes, void* cuda_stream) {
+  GV_TRY(e, {
+    if (!io) throw std::runtime_error("gimmvfi_forward_queries: io is required");
+    e->eng.forward_queries(to_problem(p), to_queries(p, queries), to_io(io), workspace, workspace_bytes, (gvStream_t)cuda_stream);
+  })
+}
+int gimmvfi_set_coord_range(gimmvfi_engine* e, double lo, double hi) {
+  GV_TRY(e, {
+    if (!std::isfinite(lo) || !std::isfinite(hi)) throw std::runtime_error("gimmvfi_set_coord_range: the range must be finite");
+    e->eng.set_coord_range(lo, hi);
+  })
+}
+
 int gimmvfi_finalize_weights_synthesis(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_synthesis(); }) }
 int gimmvfi_finalize_weights_f(gimmvfi_engine* e) { GV_TRY(e, { e->eng.finalize_weights_f(); }) }
 int gimmvfi_set_flowformer_iters(gimmvfi_engine* e, int iters) { GV_TRY(e, { if (iters < 1) throw std::runtime_error("iters must be >= 1"); e->eng.ff_iters = iters; }) }

@@ -435,6 +435,12 @@ void alt_corr_backward(Ctx& cx, const AltCorrArgs& a, const float* corr_grad, fl
 // ops_pointwise.cu
 void nchw_to_nhwc(Ctx& cx, const float* src, int64_t src_sn, int64_t src_sc, const TV& dst, float scale, float shift);
 void nhwc_to_nchw(Ctx& cx, const TV& src, float* dst, int64_t dst_sn, int64_t dst_sc, float scale, float shift, int clamp01);  // (v + shift) * scale
+// index-table stores: sample n of src goes to row rows[n] of dst (rows ride in the kernel parameters, kGatherMax per launch)
+constexpr int kGatherMax = 64;
+void nhwc_to_nchw_rows(Ctx& cx, const TV& src, float* dst, const std::vector<int>& rows, int64_t dst_sn, int64_t dst_sc, float scale, float shift,
+                       int clamp01);
+// sample_coord_input's grid for n = t.size() samples, each at its own t: coords (n,hc,wc,3) (t, y, x) and tdev (n), on the device
+void query_coords(Ctx& cx, const std::vector<float>& t, int hc, int wc, float lo, float span, float* coords, float* tdev);
 void copy_channels(Ctx& cx, const TV& src, const TV& dst);
 void frames_u8_to_padded_f32(Ctx& cx, const uint8_t* src, int n, int h, int w, float* dst_nchw, int H, int W, int pad_top, int pad_left);
 void pred_to_u8(Ctx& cx, const float* src_nchw, int n, int H, int W, uint8_t* dst, int h, int w, int pad_top, int pad_left, int bgr);
@@ -492,6 +498,7 @@ void warp_blend(Ctx& cx, const TV& img0, const TV& img1, const TV& f0, const TV&
 void multi_flow_blend(Ctx& cx, const TV& img0, const TV& img1, const TV& f0, const TV& f1, const TV& mask, const TV& res,
                       const TV& warps9, const TV& mean3);
 void combine_output(Ctx& cx, const TV& mean3, const TV& conv3, float* dst_nchw);
+void combine_output_rows(Ctx& cx, const TV& mean3, const TV& conv3, float* dst_nchw, const std::vector<int>& rows);   // image n -> dst image rows[n]
 // LPIPS (src/utils/lpips, AlexNet v0.1): conv1's input as a 4x4 space-to-depth of the padded, prepared images (dst (2n, hs, ws, 48),
 // images [in0 ; in1]), MaxPool2d(3, 2), and the head: per-row partial sums of one layer's term, then per image the 5 spatial means
 void lpips_prep(Ctx& cx, const float* in0, const float* in1, int n, int h, int w, int quantize, int normalize, const float* shift,

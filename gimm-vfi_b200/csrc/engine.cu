@@ -978,7 +978,6 @@ struct ScaleShiftK {  // y = a*x + b on a dense tensor
 
 // dst sample i <- src sample idx[i]: a clip's per-frame products into pair order.  Whole samples (padding lanes included) as 16- or
 // 4-byte words; the sample list rides in the kernel parameters, kGatherMax samples per launch.
-constexpr int kGatherMax = 64;
 struct alignas(16) Word16 { uint32_t v[4]; };
 template <class Wd> struct GatherSamplesK {
   const Wd* src; Wd* dst; int64_t words; int idx[kGatherMax];
@@ -1015,6 +1014,56 @@ static void check_problem(const Problem& p) {
     throw std::runtime_error("gimmvfi: network resolution must be a multiple of 8 and >= 128 (got " + std::to_string(H) + "x" + std::to_string(W) + ")");
   if (p.Hc != H || p.Wc != W)
     throw std::runtime_error("gimmvfi: coordinate grid must match the network resolution (frame_synthesize consumes flow_t at that size)");
+}
+
+// A query list as run() takes it.  The distinct pairs are ordered by timestep count, descending (stable), so that timestep slot k runs
+// over the prefix of the pairs that have more than k timesteps: every per-pair buffer is batch-major, and slot k works on .batch(0, B_k)
+// views.  Only the frames some query uses are read and encoded.
+struct QuerySchedule {
+  std::vector<int> frames;           // the used frames, ascending: compact frame i is caller frame frames[i]
+  Clip clip;                         // over the compact frames, pairs in slot order
+  std::vector<int> first;            // pair i's row among the distinct pairs in first-appearance order (raft_flow, nflow)
+  std::vector<std::vector<int>> q;   // pair i's queries, in query order: slot k's output row of pair i is q[i][k]
+  std::vector<float> t;              // (Q) the t of every query
+  int T = 0;                         // slots: the largest timestep count
+  int slot_pairs(int k) const { int n = 0; while (n < (int)q.size() && (int)q[n].size() > k) ++n; return n; }
+};
+
+static QuerySchedule schedule_queries(const Queries& qs) {
+  const int Q = (int)qs.src.size(), F = qs.F;
+  if (Q < 1) throw std::runtime_error("gimmvfi queries: at least one query is required");
+  if (F < 1) throw std::runtime_error("gimmvfi queries: at least one frame is required");
+  if ((int)qs.tgt.size() != Q || (int)qs.t.size() != Q) throw std::runtime_error("gimmvfi queries: src, tgt and t differ in length");
+  std::map<std::pair<int, int>, int> pair_of;   // (src, tgt) -> distinct pair, first-appearance order
+  std::vector<std::pair<int, int>> pairs;
+  std::vector<std::vector<int>> q;
+  for (int i = 0; i < Q; ++i) {
+    const int a = qs.src[i], b = qs.tgt[i];
+    if (a < 0 || a >= F || b < 0 || b >= F)
+      throw std::runtime_error("gimmvfi queries: query " + std::to_string(i) + " = (" + std::to_string(a) + ", " + std::to_string(b) +
+                               ") indexes outside the " + std::to_string(F) + " frames");
+    const float t = qs.t[i];
+    if (!std::isfinite(t) || !(t > 0.f && t < 1.f))   // the AMT lookup scales by 1/t and 1/(1-t) (gimmvfi_r.py:494-507)
+      throw std::runtime_error("gimmvfi queries: query " + std::to_string(i) + " has t = " + std::to_string(t) + "; t must lie strictly inside (0, 1)");
+    auto it = pair_of.find({a, b});
+    if (it == pair_of.end()) { it = pair_of.emplace(std::make_pair(a, b), (int)pairs.size()).first; pairs.push_back({a, b}); q.emplace_back(); }
+    q[it->second].push_back(i);
+  }
+  std::vector<int> order(pairs.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
+  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return q[x].size() > q[y].size(); });
+  QuerySchedule s;
+  std::vector<int> compact(F, -1);
+  for (const auto& ab : pairs) compact[ab.first] = compact[ab.second] = 0;
+  for (int f = 0; f < F; ++f) if (compact[f] == 0) { compact[f] = (int)s.frames.size(); s.frames.push_back(f); }
+  s.clip.F = (int)s.frames.size();
+  for (int d : order) {
+    s.clip.src.push_back(compact[pairs[d].first]); s.clip.tgt.push_back(compact[pairs[d].second]);
+    s.first.push_back(d); s.q.push_back(q[d]);
+  }
+  s.t = qs.t;
+  s.T = (int)s.q[0].size();
+  return s;
 }
 
 // RAFT.forward (raft/raft.py:100-169) over F prepared frames and a list of (source, target) pairs, batched on the N axis.  fnet runs once
@@ -1183,7 +1232,9 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   tap("raft.net_final", hcur);
 }
 
-void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin, const Clip* clip) {
+void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin, const Clip* clip, const QuerySchedule* qs) {
+  Problem P = P0;
+  if (qs) { clip = &qs->clip; P.B = (int)qs->clip.src.size(); P.T = qs->T; }   // a query list: its distinct pairs and slots
   check_problem(P);
   Net N{*this, cx};
   Arena& A = cx.arena;
@@ -1216,9 +1267,14 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
   for (int s = 0; s < 2 * B; ++s) pslot[s] = fslot[esrc[s]];
 
   // ------------------------------------------------------------ inputs
-  // frames as NHWC, stacked [I0 batch ; I1 batch] (a clip: its frames in order)
+  // frames as NHWC, stacked [I0 batch ; I1 batch] (a clip: its frames in order; a query list: its used frames, in runs of consecutive ones)
   TV full01 = A.tensor(NF, Hf, Wf, 3, 4);
-  if (clip)
+  if (qs)
+    for (int i0 = 0, i1; i0 < NF; i0 = i1) {
+      for (i1 = i0 + 1; i1 < NF && qs->frames[i1] == qs->frames[i1 - 1] + 1;) ++i1;
+      nchw_to_nhwc(cx, io.img_xs + (int64_t)qs->frames[i0] * 3 * Hf * Wf, (int64_t)3 * Hf * Wf, (int64_t)Hf * Wf, full01.batch(i0, i1 - i0), 1.f, 0.f);
+    }
+  else if (clip)
     nchw_to_nhwc(cx, io.img_xs, (int64_t)3 * Hf * Wf, (int64_t)Hf * Wf, full01, 1.f, 0.f);
   else
     for (int f = 0; f < 2; ++f)
@@ -1307,9 +1363,14 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
     run_raft(cx, N, r);
     if (!debug_) A.release(mk);
   }
-  if (io.raft_flow)
-    for (int j = 0; j < 2; ++j)
-      nhwc_to_nchw(cx, flow_up.batch(j * B, B), io.raft_flow + (int64_t)j * H * W, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
+  // (B,2,2,H,W) per-pair outputs from [direction 0 ; direction 1] samples; a query list's rows are its distinct pairs in first-appearance order
+  auto store_pairs = [&](const TV& both, float* dst) {
+    for (int j = 0; j < 2; ++j) {
+      if (qs) nhwc_to_nchw_rows(cx, both.batch(j * B, B), dst + (int64_t)j * H * W, qs->first, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
+      else nhwc_to_nchw(cx, both.batch(j * B, B), dst + (int64_t)j * H * W, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
+    }
+  };
+  if (io.raft_flow) store_pairs(flow_up, io.raft_flow);
 
   // Everything downstream of RAFT tolerates TF32 operands (DESIGN.md precision plan).
   cx.tc = tc_mode_ >= 1; cx.tc_split = false;
@@ -1330,23 +1391,35 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
   }
   // the bidirectional volume only feeds TF32 layers (AMT update blocks) -> plain TF32 is at their input precision
   // Few interpolated frames per pair (T <= corr_direct_max_t): no volume at all - the lookup computes the dot products its window needs
-  // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.
+  // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.  A query list decides per pair, as that pair's
+  // own forward would: its pairs are sorted by timestep count, so the pyramid pairs are a prefix [0, Bp) and the direct ones [Bp, B).
   Pyramid bpyr{}; CorrFeat bfeat{};
   constexpr int corr_direct_max_t = 2;
-  const bool corr_direct = tc_mode_ >= 1 && T <= corr_direct_max_t && fproj.c == 256 && h >= 16 && w >= 16;
-  if (corr_direct) {
-    TV Fl = fproj;
+  const bool direct_ok = tc_mode_ >= 1 && fproj.c == 256 && h >= 16 && w >= 16;
+  int Bp = direct_ok && T <= corr_direct_max_t ? 0 : B;
+  if (qs && direct_ok) { Bp = 0; while (Bp < B && (int)qs->q[Bp].size() > corr_direct_max_t) ++Bp; }
+  const int Bd = B - Bp;
+  if (Bd > 0) {
+    // half features of the direct pairs' samples, [sources ; targets]: compact sample i < Bd is pair Bp + i's source, Bd + i its target
+    std::vector<TV> runs = {fproj};
+    if (Bp > 0) runs = {fproj.batch(Bp, Bd), fproj.batch(B + Bp, Bd)};
     bfeat.c = 256; bfeat.scale = 1.0f / std::sqrt((float)fproj.c);
     for (int l = 0; l < 4; ++l) {
-      bfeat.h[l] = Fl.h; bfeat.w[l] = Fl.w;
-      void* hp = A.alloc_f(((size_t)Fl.pixels() * Fl.c + 1) / 2);
-      features_to_half(cx, Fl, hp);
-      bfeat.lvl[l] = static_cast<const uint16_t*>(hp);
-      if (l < 3) { TV nx = A.tensor(2 * B, Fl.h / 2, Fl.w / 2, Fl.c); avgpool2_features(cx, Fl, nx); Fl = nx; }
+      bfeat.h[l] = runs[0].h; bfeat.w[l] = runs[0].w;
+      const size_t per = (size_t)runs[0].h * runs[0].w * runs[0].c;
+      uint16_t* hp = reinterpret_cast<uint16_t*>(A.alloc_f(((size_t)2 * Bd * per + 1) / 2));
+      for (size_t r = 0, n0 = 0; r < runs.size(); n0 += runs[r].n, ++r) features_to_half(cx, runs[r], hp + n0 * per);
+      bfeat.lvl[l] = hp;
+      if (l < 3) {
+        TV nx = A.tensor(2 * Bd, runs[0].h / 2, runs[0].w / 2, runs[0].c);
+        for (size_t r = 0, n0 = 0; r < runs.size(); n0 += runs[r].n, ++r) avgpool2_features(cx, runs[r], nx.batch((int)n0, runs[r].n));
+        runs = {nx};
+      }
     }
-  } else {
-    std::vector<int> src(2 * B), tgt(2 * B);   // [f0 ; f1] against [f1 ; f0]
-    for (int s = 0; s < 2 * B; ++s) { src[s] = s; tgt[s] = s < B ? s + B : s - B; }
+  }
+  if (Bp > 0) {
+    std::vector<int> src(2 * Bp), tgt(2 * Bp);   // [f0 ; f1] against [f1 ; f0] of the pyramid pairs
+    for (int s = 0; s < Bp; ++s) { src[s] = tgt[Bp + s] = s; tgt[s] = src[Bp + s] = B + s; }
     bpyr = build_pyramid(cx, fproj, src, tgt, tc_mode_ >= 1 ? 1 : 0);   // gimmvfi_r.py:133, raft/corr.py:23-44
   }
   auto bfeat_of = [&](int sample0) {
@@ -1402,50 +1475,68 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
   }
   TV nf = A.tensor(2 * B, H, W, 2);
   normalize_flow_pair(cx, f01, f10, scaler, nf.batch(0, B), nf.batch(B, B));
-  if (io.nflow)
-    for (int j = 0; j < 2; ++j)
-      nhwc_to_nchw(cx, nf.batch(j * B, B), io.nflow + (int64_t)j * H * W, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
+  if (io.nflow) store_pairs(nf, io.nflow);
   TV wts = A.tensor(2 * B, H, W, 1);
   TV X64 = A.tensor(B, H, W, 64);   // [lat0 | lat1 | splat0 | splat1]
   gimm_encode(N, nf, f01, f10, wts, X64);
 
   // ------------------------------------------------------------ per-timestep: GIMM decode + frame synthesis
+  // A query list's slot ti runs over its first Bk pairs (those with more than ti timesteps): every per-pair buffer below is batch-major,
+  // so the slot works on .batch(0, Bk) views of the first direction and .batch(B, Bk) of the second.  Its coordinates and t are made
+  // here, and its outputs are stored at the rows of its queries.
   TV grid_flow = A.tensor(B, h, w, 4);   // flow_4_lr = cat(fl0, fl1)
   const size_t t_mark = A.mark();
   for (int ti = 0; ti < T; ++ti) {
     A.release(t_mark);
     // debug taps of the per-timestep tensors are taken at the last timestep: nothing overwrites them after it
     const bool last = ti == T - 1;
-    const float* tdev = io.t + (int64_t)ti * B;
-    TV ninr = A.tensor(B, H, W, 2);
-    gimm_decode(N, X64, f01, f10, wts, tdev, io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3, ninr, last);
-    if (io.ninrflow) nhwc_to_nchw(cx, ninr, io.ninrflow + (int64_t)ti * B * 2 * H * W, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
-    TV flow_t = A.tensor(B, H, W, 2);
+    const int Bk = qs ? qs->slot_pairs(ti) : B;
+    const float* tdev = io.t ? io.t + (int64_t)ti * B : nullptr;
+    const float* coords_t = io.coords ? io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3 : nullptr;
+    std::vector<int> rows;   // a query list: the output row (query) of each of the slot's samples
+    if (qs) {
+      std::vector<float> ts;
+      for (int b = 0; b < Bk; ++b) { rows.push_back(qs->q[b][ti]); ts.push_back(qs->t[qs->q[b][ti]]); }
+      float* tq = A.alloc_f(std::max(Bk, 64));
+      float* cq = A.alloc_f((size_t)Bk * P.Hc * P.Wc * 3);
+      if (!cx.dry) query_coords(cx, ts, P.Hc, P.Wc, coord_lo_, coord_span_, cq, tq);
+      tdev = tq; coords_t = cq;
+      if (last) tap("query.coords", make_tv(cq, Bk, P.Hc, P.Wc, 3));
+    }
+    // per-timestep outputs (ti, B, ...): rows ti * B + b; a query list's: the rows of its queries
+    auto store = [&](const TV& src, float* dst, int64_t sn, int64_t sc, float scale, float shift, int clamp01) {
+      if (qs) nhwc_to_nchw_rows(cx, src, dst, rows, sn, sc, scale, shift, clamp01);
+      else nhwc_to_nchw(cx, src, dst + (int64_t)ti * B * sn, sn, sc, scale, shift, clamp01);
+    };
+    TV ninr = A.tensor(Bk, H, W, 2);
+    gimm_decode(N, X64.batch(0, Bk), f01.batch(0, Bk), f10.batch(0, Bk), wts.batch(0, Bk), wts.batch(B, Bk), tdev, coords_t, ninr, last);
+    if (io.ninrflow) store(ninr, io.ninrflow, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
+    TV flow_t = A.tensor(Bk, H, W, 2);
     unnormalize_flow(cx, ninr, scaler, flow_t);
-    if (io.flowt) nhwc_to_nchw(cx, flow_t, io.flowt + (int64_t)ti * B * 2 * H * W, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
+    if (io.flowt) store(flow_t, io.flowt, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
 
     // ---- frame_synthesize (gimmvfi_r.py:222-322)
-    TV s0 = syn.batch(0, B), s1 = syn.batch(B, B);
-    TV ft0 = A.tensor(B, H, W, 2), ft1 = A.tensor(B, H, W, 2);
+    TV s0 = syn.batch(0, Bk), s1 = syn.batch(B, Bk);
+    TV ft0 = A.tensor(Bk, H, W, 2), ft1 = A.tensor(Bk, H, W, 2);
     scale_flow_t(cx, flow_t, tdev, ft0, ft1);
     // NewInitDecoder (fi_components.py:255-276)
-    TV fin = A.tensor(B, H4, W4, 272);
+    TV fin = A.tensor(Bk, H4, W4, 272);
     TV f0in = fin.slice(256, 2), f1in = fin.slice(258, 2);
     resize_bilinear(cx, ft0, f0in, 4.f, 4.f, 0.25f, 0, ACT_NONE);
     resize_bilinear(cx, ft1, f1in, 4.f, 4.f, 0.25f, 0, ACT_NONE);
-    backwarp(cx, fup4.batch(0, B), f0in, fin.slice(0, 128));
-    backwarp(cx, fup4.batch(B, B), f1in, fin.slice(128, 128));
+    backwarp(cx, fup4.batch(0, Bk), f0in, fin.slice(0, 128));
+    backwarp(cx, fup4.batch(B, Bk), f1in, fin.slice(128, 128));
     resize_bilinear(cx, s0, fin.slice(260, 3), 4.f, 4.f, 1.f, 0, ACT_NONE);
     resize_bilinear(cx, s1, fin.slice(263, 3), 4.f, 4.f, 1.f, 0, ACT_NONE);
     backwarp(cx, fin.slice(260, 3), f0in, fin.slice(266, 3));
     backwarp(cx, fin.slice(263, 3), f1in, fin.slice(269, 3));
-    TV x4 = half_chains(cx) ? A.tensor_h(B, H4, W4, 128) : A.tensor(B, H4, W4, 128);   // (mode 4: the H/4 residual trunk in half too)
+    TV x4 = half_chains(cx) ? A.tensor_h(Bk, H4, W4, 128) : A.tensor(Bk, H4, W4, 128);   // (mode 4: the H/4 residual trunk in half too)
     N.convrelu("amt_init_decoder.convblock.0", fin, x4);
     for (int k = 1; k <= 3; ++k) resblock(N, "amt_init_decoder.convblock." + std::to_string(k), x4, 128, 64);
-    TV o136 = A.tensor(B, H4, W4, 133, 136);
+    TV o136 = A.tensor(Bk, H4, W4, 133, 136);
     N.conv("amt_init_decoder.convblock.4", x4, o136);
     TV ft_4 = o136.slice(0, 128);
-    TV fl4 = A.tensor(B, H4, W4, 4), mask4 = A.tensor(B, H4, W4, 1);
+    TV fl4 = A.tensor(Bk, H4, W4, 4), mask4 = A.tensor(Bk, H4, W4, 1);
     flow_mask_split(cx, o136, f0in, f1in, fl4.slice(0, 2), fl4.slice(2, 2), mask4);
     if (last) {   // (ft_4 / fl4 are updated in place by the update blocks: snapshots)
       tap("syn.fin4", fin); tap("syn.mask4_init", mask4);
@@ -1454,62 +1545,65 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
     // warp_w_mask(scale=4) -> img_warp_4 (aux output, gimmvfi_r.py:259-261)
     if (io.img_warp_4) {
       const size_t mk = A.mark();
-      TV a0 = A.tensor(B, H, W, 2), a1 = A.tensor(B, H, W, 2), am = A.tensor(B, H, W, 1), wb = A.tensor(B, H, W, 3, 4);
+      TV a0 = A.tensor(Bk, H, W, 2), a1 = A.tensor(Bk, H, W, 2), am = A.tensor(Bk, H, W, 1), wb = A.tensor(Bk, H, W, 3, 4);
       resize_bilinear(cx, fl4.slice(0, 2), a0, 0.25f, 0.25f, 4.f, 0, ACT_NONE);
       resize_bilinear(cx, fl4.slice(2, 2), a1, 0.25f, 0.25f, 4.f, 0, ACT_NONE);
       resize_bilinear(cx, mask4, am, 0.25f, 0.25f, 1.f, 0, ACT_SIGMOID);
       warp_blend(cx, s0, s1, a0, a1, am, wb);
-      nhwc_to_nchw(cx, wb, io.img_warp_4 + (int64_t)ti * B * 3 * H * W, (int64_t)3 * H * W, (int64_t)H * W, 0.5f, 1.0f, 1);
+      store(wb, io.img_warp_4, (int64_t)3 * H * W, (int64_t)H * W, 0.5f, 1.0f, 1);
       A.release(mk);
     }
     // _amt_corr_scale_lookup(downsample=2)  (gimmvfi_r.py:494-507)
-    TV corr648 = A.tensor(B, h, w, 648);
+    TV corr648 = A.tensor(Bk, h, w, 648);
     {
-      resize_bilinear(cx, fl4, grid_flow, 2.f, 2.f, 0.5f, 0, ACT_NONE);
-      TV cA = A.tensor(B, h, w, 2), cB = A.tensor(B, h, w, 2);
-      lookup_coords(cx, grid_flow.slice(2, 2), tdev, 0, cA);  // coord + flow1 * 1/(1-t) -> volume
-      lookup_coords(cx, grid_flow.slice(0, 2), tdev, 1, cB);  // coord + flow0 * 1/t     -> transposed volume
-      if (corr_direct) {   // rows = frame 0's pixels against frame 1's features, and the transposed volume's counterpart
-        corr_lookup_direct(cx, fproj.batch(0, B), bfeat_of(B), cA, corr648.slice(0, 324));
-        corr_lookup_direct(cx, fproj.batch(B, B), bfeat_of(0), cB, corr648.slice(324, 324));
-      } else {
-        corr_lookup(cx, bpyr.view(0), cA, corr648.slice(0, 324));
-        corr_lookup(cx, bpyr.view(B), cB, corr648.slice(324, 324));
+      TV gf = grid_flow.batch(0, Bk);
+      resize_bilinear(cx, fl4, gf, 2.f, 2.f, 0.5f, 0, ACT_NONE);
+      TV cA = A.tensor(Bk, h, w, 2), cB = A.tensor(Bk, h, w, 2);
+      lookup_coords(cx, gf.slice(2, 2), tdev, 0, cA);  // coord + flow1 * 1/(1-t) -> volume
+      lookup_coords(cx, gf.slice(0, 2), tdev, 1, cB);  // coord + flow0 * 1/t     -> transposed volume
+      const int np = std::min(Bp, Bk), nd = Bk - np;
+      if (np > 0) {
+        corr_lookup(cx, bpyr.view(0), cA.batch(0, np), corr648.batch(0, np).slice(0, 324));
+        corr_lookup(cx, bpyr.view(Bp), cB.batch(0, np), corr648.batch(0, np).slice(324, 324));
+      }
+      if (nd > 0) {   // rows = frame 0's pixels against frame 1's features, and the transposed volume's counterpart
+        corr_lookup_direct(cx, fproj.batch(Bp, nd), bfeat_of(Bd), cA.batch(np, nd), corr648.batch(np, nd).slice(0, 324));
+        corr_lookup_direct(cx, fproj.batch(B + Bp, nd), bfeat_of(0), cB.batch(np, nd), corr648.batch(np, nd).slice(324, 324));
       }
     }
-    amt_update(N, "amt_update4_low", true, ft_4, fl4, grid_flow, corr648);
+    amt_update(N, "amt_update4_low", true, ft_4, fl4, grid_flow.batch(0, Bk), corr648);
     if (last) { tap("syn.corr648", corr648); tap_copy(cx, "syn.ft4_low", ft_4); tap_copy(cx, "syn.fl4_low", fl4); }
     {
-      TV corr_hi = A.tensor(B, H4, W4, 648);
+      TV corr_hi = A.tensor(Bk, H4, W4, 648);
       resize_bilinear(cx, corr648, corr_hi, 0.5f, 0.5f, 1.f, 0, ACT_NONE);  // gimmvfi_r.py:274
       amt_update(N, "amt_update4_high", false, ft_4, fl4, fl4, corr_hi);
       if (last) tap("syn.corr_4_hi", corr_hi);
     }
     if (last) { tap("syn.ft_4", ft_4); tap("syn.fl4", fl4); tap("syn.mask4", mask4); }
-    if (io.flowt0_4) nhwc_to_nchw(cx, fl4.slice(0, 2), io.flowt0_4 + (int64_t)ti * B * 2 * H4 * W4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
-    if (io.flowt1_4) nhwc_to_nchw(cx, fl4.slice(2, 2), io.flowt1_4 + (int64_t)ti * B * 2 * H4 * W4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
+    if (io.flowt0_4) store(fl4.slice(0, 2), io.flowt0_4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
+    if (io.flowt1_4) store(fl4.slice(2, 2), io.flowt1_4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
 
     // NewMultiFlowDecoder (fi_components.py:307-340)
-    TV F0 = A.tensor(B, H, W, 6, 8), F1 = A.tensor(B, H, W, 6, 8), Mk = A.tensor(B, H, W, 3, 4), Rs = A.tensor(B, H, W, 9, 12);
+    TV F0 = A.tensor(Bk, H, W, 6, 8), F1 = A.tensor(Bk, H, W, 6, 8), Mk = A.tensor(Bk, H, W, 3, 4), Rs = A.tensor(Bk, H, W, 9, 12);
     // debug snapshots of the concat, the fp32 flows / mask and convblock.4's output: allocated here, outside the block that frees them
     const bool snap = debug_ && last;
-    TV fin1_snap = snap ? A.tensor(B, H, W, 273) : TV(), aux5_snap = snap && half_chains(cx) ? A.tensor(B, H, W, 5) : TV();
-    TV o24_snap = snap ? A.tensor(B, H, W, 24) : TV();
+    TV fin1_snap = snap ? A.tensor(Bk, H, W, 273) : TV(), aux5_snap = snap && half_chains(cx) ? A.tensor(Bk, H, W, 5) : TV();
+    TV o24_snap = snap ? A.tensor(Bk, H, W, 24) : TV();
     {
       const size_t mk = A.mark();
       // precision mode 4: the 273-channel concat buffer itself is half precision (written by the half-aware resize / backwarp /
       // copy kernels); the up-sampled flows and mask are additionally kept in fp32 (they drive the warps and the output heads)
       const bool hs = half_chains(cx);
-      TV fin1 = hs ? A.tensor_h(B, H, W, 273, 280) : A.tensor(B, H, W, 273, 276);
-      TV aux5 = hs ? A.tensor(B, H, W, 5, 8) : TV();
+      TV fin1 = hs ? A.tensor_h(Bk, H, W, 273, 280) : A.tensor(Bk, H, W, 273, 276);
+      TV aux5 = hs ? A.tensor(Bk, H, W, 5, 8) : TV();
       TV fl0 = hs ? aux5.slice(0, 2) : fin1.slice(256, 2), fl1 = hs ? aux5.slice(2, 2) : fin1.slice(258, 2), mk1 = hs ? aux5.slice(4, 1) : fin1.slice(260, 1);
       resize_bilinear(cx, fl4.slice(0, 2), fl0, 0.25f, 0.25f, 4.f, 0, ACT_NONE);
       resize_bilinear(cx, fl4.slice(2, 2), fl1, 0.25f, 0.25f, 4.f, 0, ACT_NONE);
       resize_bilinear(cx, ft_4, fin1.slice(0, 128), 0.25f, 0.25f, 1.f, 0, ACT_NONE);
       resize_bilinear(cx, mask4, mk1, 0.25f, 0.25f, 1.f, 0, ACT_NONE);
       if (hs) copy_channels(cx, aux5.slice(0, 5), fin1.slice(256, 5));
-      backwarp(cx, fup1.batch(0, B), fl0, fin1.slice(128, 64));
-      backwarp(cx, fup1.batch(B, B), fl1, fin1.slice(192, 64));
+      backwarp(cx, fup1.batch(0, Bk), fl0, fin1.slice(128, 64));
+      backwarp(cx, fup1.batch(B, Bk), fl1, fin1.slice(192, 64));
       copy_channels(cx, s0, fin1.slice(261, 3));
       copy_channels(cx, s1, fin1.slice(264, 3));
       backwarp(cx, s0, fl0, fin1.slice(267, 3));
@@ -1520,10 +1614,10 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
       }
       // precision mode 3: the 256-channel residual trunk (9 of the 10 heaviest launches) is stored in fp16 and runs on the
       // f16 tensor-core path (same 10-bit mantissa as TF32, half the bytes per operand, twice the MMA rate)
-      TV x1 = (cx.tc && tc_mode_ >= 3) ? A.tensor_h(B, H, W, 256) : A.tensor(B, H, W, 256);
+      TV x1 = (cx.tc && tc_mode_ >= 3) ? A.tensor_h(Bk, H, W, 256) : A.tensor(Bk, H, W, 256);
       N.convrelu("amt_final_decoder.convblock.0", fin1, x1);
       for (int k = 1; k <= 3; ++k) resblock(N, "amt_final_decoder.convblock." + std::to_string(k), x1, 256, 64);
-      TV o24 = A.tensor(B, H, W, 24);
+      TV o24 = A.tensor(Bk, H, W, 24);
       N.conv("amt_final_decoder.convblock.4", x1, o24);
       if (snap) tap_copy_to(cx, "syn.o24", o24, o24_snap);
       final_heads(cx, o24, fl0, fl1, mk1, F0, F1, Mk, Rs);
@@ -1532,7 +1626,7 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
     if (last) { tap("syn.F0", F0); tap("syn.F1", F1); tap("syn.Mk", Mk); tap("syn.Rs", Rs); }
     TV F0f = F0, F1f = F1, Mkf = Mk, Rsf = Rs;
     if (ds) {  // gimmvfi_r.py:294-303
-      F0f = A.tensor(B, Hf, Wf, 6, 8); F1f = A.tensor(B, Hf, Wf, 6, 8); Mkf = A.tensor(B, Hf, Wf, 3, 4); Rsf = A.tensor(B, Hf, Wf, 9, 12);
+      F0f = A.tensor(Bk, Hf, Wf, 6, 8); F1f = A.tensor(Bk, Hf, Wf, 6, 8); Mkf = A.tensor(Bk, Hf, Wf, 3, 4); Rsf = A.tensor(Bk, Hf, Wf, 9, 12);
       // (views widened to the pixel stride: the padding lanes ride along so that the 16-byte form of the kernel applies - 6 / 3 / 9
       //  channels are not multiples of 4; the scalar form was 12.6 ms of the 4K configuration's 208)
       auto wide = [](TV t) { t.c = t.ld; return t; };
@@ -1542,15 +1636,16 @@ void Engine::run(Ctx& cx, const Problem& P, const IO& io, const FlowInputs* fin,
       resize_bilinear(cx, wide(Rs), wide(Rsf), rinv, rinv, 1.f, 0, ACT_NONE);
       if (last) { tap("syn.F0f", F0f); tap("syn.F1f", F1f); tap("syn.Mkf", Mkf); tap("syn.Rsf", Rsf); }
     }
-    if (io.flowt0_1) nhwc_to_nchw(cx, F0f, io.flowt0_1 + (int64_t)ti * B * 6 * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
-    if (io.flowt1_1) nhwc_to_nchw(cx, F1f, io.flowt1_1 + (int64_t)ti * B * 6 * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
+    if (io.flowt0_1) store(F0f, io.flowt0_1, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
+    if (io.flowt1_1) store(F1f, io.flowt1_1, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
     // multi_flow_combine + amt_comb_block at FULL resolution (fi_components.py:57-94)
     {
-      TV w9 = A.tensor(B, Hf, Wf, 9, 12), mean3 = A.tensor(B, Hf, Wf, 3, 4), c18 = A.tensor(B, Hf, Wf, 18, 20), c3 = A.tensor(B, Hf, Wf, 3, 4);
-      multi_flow_blend(cx, synf.batch(0, B), synf.batch(B, B), F0f, F1f, Mkf, Rsf, w9, mean3);
+      TV w9 = A.tensor(Bk, Hf, Wf, 9, 12), mean3 = A.tensor(Bk, Hf, Wf, 3, 4), c18 = A.tensor(Bk, Hf, Wf, 18, 20), c3 = A.tensor(Bk, Hf, Wf, 3, 4);
+      multi_flow_blend(cx, synf.batch(0, Bk), synf.batch(B, Bk), F0f, F1f, Mkf, Rsf, w9, mean3);
       N.conv7x("amt_comb_block.0", w9, c18, ACT_PRELU, N.V("amt_comb_block.1.weight"));
       N.conv7x("amt_comb_block.2", c18, c3);
-      combine_output(cx, mean3, c3, io.imgt_pred + (int64_t)ti * B * 3 * Hf * Wf);
+      if (qs) combine_output_rows(cx, mean3, c3, io.imgt_pred, rows);
+      else combine_output(cx, mean3, c3, io.imgt_pred + (int64_t)ti * B * 3 * Hf * Wf);
       if (last) { tap("syn.w9", w9); tap("syn.mean3", mean3); tap("syn.c3", c3); }
     }
   }
@@ -1589,8 +1684,8 @@ void Engine::gimm_encode(Net& N, const TV& nf /*2B: [nf01; nf10]*/, const TV& f0
 }
 
 // one timestep: forward splat of both latents to time t, latent refiner, HypoNet -> normalised flow ninr (B,Hc,Wc,2) on the coordinate grid
-void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, const TV& wts, const float* tdev, const float* coords_t,
-                         const TV& ninr, bool tap_it) {
+void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, const TV& w01, const TV& w10, const float* tdev,
+                         const float* coords_t, const TV& ninr, bool tap_it) {
   Ctx& cx = N.cx; Arena& A = cx.arena;
   const int B = f01.n, H = f01.h, W = f01.w;
   const size_t mk0 = A.mark();
@@ -1599,13 +1694,13 @@ void Engine::gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, co
   const int fwarp = motion_.fwarp;
   if (fwarp == SPLAT_SUM) {   // the plain sum is the result: accumulated straight into the latent buffer
     fill(cx, X64.slice(32, 32), 0.f);
-    softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, wts.batch(0, B), tdev, 0, X64.slice(32, 16), SPLAT_SUM);
-    softsplat_accumulate_mode(cx, X64.slice(16, 16), f10, wts.batch(B, B), tdev, 1, X64.slice(48, 16), SPLAT_SUM);
+    softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, w01, tdev, 0, X64.slice(32, 16), SPLAT_SUM);
+    softsplat_accumulate_mode(cx, X64.slice(16, 16), f10, w10, tdev, 1, X64.slice(48, 16), SPLAT_SUM);
   } else {
     TV acc = A.tensor(2 * B, H, W, 17, 20);
     if (!cx.dry) dev_memset(acc.p, 0, (size_t)2 * B * H * W * 20 * sizeof(float), cx.stream);
-    softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, wts.batch(0, B), tdev, 0, acc.batch(0, B), fwarp);
-    softsplat_accumulate_mode(cx, X64.slice(16, 16), f10, wts.batch(B, B), tdev, 1, acc.batch(B, B), fwarp);
+    softsplat_accumulate_mode(cx, X64.slice(0, 16), f01, w01, tdev, 0, acc.batch(0, B), fwarp);
+    softsplat_accumulate_mode(cx, X64.slice(16, 16), f10, w10, tdev, 1, acc.batch(B, B), fwarp);
     softsplat_normalize(cx, acc.batch(0, B), X64.slice(32, 16));
     softsplat_normalize(cx, acc.batch(B, B), X64.slice(48, 16));
   }
@@ -1696,7 +1791,7 @@ void Engine::run_gimm(Ctx& cx, const Problem& P, const GimmIO& io) {
   gimm_encode(N, nf, f01, f10, wts, X64);
   TV ninr = A.tensor(B, Hc, Wc, 2);
   for (int ti = 0; ti < T; ++ti) {
-    gimm_decode(N, X64, f01, f10, wts, io.t + (int64_t)ti * B, io.coords + (int64_t)ti * B * Hc * Wc * 3, ninr, ti == T - 1);
+    gimm_decode(N, X64, f01, f10, wts.batch(0, B), wts.batch(B, B), io.t + (int64_t)ti * B, io.coords + (int64_t)ti * B * Hc * Wc * 3, ninr, ti == T - 1);
     nhwc_to_nchw(cx, ninr, io.out + (int64_t)ti * B * 2 * Hc * Wc, (int64_t)2 * Hc * Wc, (int64_t)Hc * Wc, 1.f, 0.f, 0);
   }
 }
@@ -1842,6 +1937,23 @@ void Engine::forward_clip(const Problem& p, const Clip& c, const IO& io, void* w
   need(Entry::Interpolate);
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: frames, coords, t and imgt_pred are required");
   launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, nullptr, &c); });
+}
+
+size_t Engine::plan_queries(const Problem& p, const Queries& q) {
+  need(Entry::Interpolate);
+  const QuerySchedule s = schedule_queries(q);
+  IO io = fake_io();
+  io.coords = io.t = nullptr;
+  return dry_run([&](Ctx& cx) { run(cx, p, io, nullptr, nullptr, &s); });
+}
+
+// (eager, as forward_clip)
+void Engine::forward_queries(const Problem& p, const Queries& q, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
+  need(Entry::Interpolate);
+  if (!io.img_xs || !io.imgt_pred) throw std::runtime_error("gimmvfi: frames and imgt_pred are required");
+  if (io.coords || io.t) throw std::runtime_error("gimmvfi: a query list's coordinates and t are made by the engine; io.coords and io.t must be null");
+  const QuerySchedule s = schedule_queries(q);
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, nullptr, nullptr, &s); });
 }
 
 // ---------------------------------------------------------------------------

@@ -47,6 +47,16 @@ struct Clip {
   std::vector<int> src, tgt;
 };
 
+// A query list (Engine::forward_queries): F frames (IO::img_xs (F,3,Hf,Wf)) and Q queries, query q interpolating from frame src[q] to
+// frame tgt[q] at t[q] in (0, 1).  Queries with the same (src, tgt) are the timesteps of one pair, in query order.  Per-timestep outputs
+// are (Q, ...) in query order; raft_flow / nflow are (P, ...) over the distinct pairs in first-appearance order.
+struct Queries {
+  int F = 0;
+  std::vector<int> src, tgt;
+  std::vector<float> t;
+};
+struct QuerySchedule;   // engine.cu: the slot schedule of a query list
+
 // Outputs of an EXTERNAL bidirectional flow estimator at the network resolution (GIMM-VFI-F: FlowFormer, gimmvfi_f.py:114-138) in the
 // reference's NCHW layouts; with these the engine runs everything downstream of cal_bidirection_flow (forward_from_flow)
 struct FlowInputs {
@@ -181,6 +191,14 @@ class Engine {
   // with B = 1 on (frames[src[p]], frames[tgt[p]]).  The plan holds for this clip's pair list.
   size_t plan_clip(const Problem& p, const Clip& c);
   void forward_clip(const Problem& p, const Clip& c, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream);
+  // GIMM-VFI-R / -F over a query list: each pair's estimator, encoders and feature upsampling run once, as in forward_clip, and each
+  // pair is interpolated at its own timesteps.  The problem supplies Hf, Wf, ds, Hc and Wc (its B and T are ignored); the engine makes
+  // the coordinates and t itself (io.coords and io.t must be null).  The plan depends on the frame count, the distinct pairs and their
+  // timestep counts, not on the t values.
+  size_t plan_queries(const Problem& p, const Queries& q);
+  void forward_queries(const Problem& p, const Queries& q, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream);
+  // the coordinate range of the query grids (the model's coord_range; sample_coord_input's arithmetic in float32)
+  void set_coord_range(double lo, double hi) { coord_lo_ = (float)lo; coord_span_ = (float)(hi - lo); }
   int64_t last_launches() const { return launches_; }
   // CUDA graphs: forward() records the launch sequence of a (problem, buffers, mode) combination the SECOND time it sees it and
   // replays the instantiated graph afterwards - one cudaGraphLaunch instead of ~550 kernel launches and ~1000 host-side tensor-map
@@ -234,7 +252,7 @@ class Engine {
   void prefix_flow_estimator(std::initializer_list<const char*> children);
   size_t dry_run(const std::function<void(Ctx&)>& run);
   void launch(void* workspace, size_t workspace_bytes, gvStream_t stream, const std::function<void(Ctx&)>& run);
-  void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr, const Clip* clip = nullptr);
+  void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr, const Clip* clip = nullptr, const QuerySchedule* qs = nullptr);
   void finalize_decoders();
   void finalize_flowformer();
   void pack_patch_conv(const std::string& name);
@@ -254,8 +272,9 @@ class Engine {
   void finalize_gimm_part();
   void run_lpips(Ctx& cx, int n, int h, int w, const LpipsIO& io);
   void gimm_encode(Net& N, const TV& nf, const TV& f01, const TV& f10, const TV& wts, const TV& X64);
-  void gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, const TV& wts, const float* tdev, const float* coords_t, const TV& ninr,
-                   bool tap_it);
+  // w01 / w10: the splat weights of the two directions
+  void gimm_decode(Net& N, const TV& X64, const TV& f01, const TV& f10, const TV& w01, const TV& w10, const float* tdev, const float* coords_t,
+                   const TV& ninr, bool tap_it);
   ConvW pack_conv(const std::string& name, const std::string& bn = "", float out_scale = 1.f, const std::vector<int>* perm = nullptr);
   const float* upload(const std::vector<float>& v);
   const float* vec(const std::string& key);
@@ -297,6 +316,7 @@ class Engine {
   const float* g9_ = nullptr; const float* alpha_fe_ = nullptr; const float* alpha_v_ = nullptr;
   MotionConfig motion_next_;   // set_motion_config
   MotionConfig motion_;        // what the packed HypoNet weights were built with (finalize_gimm_part); the forwards read this one
+  float coord_lo_ = -1.f, coord_span_ = 2.f;   // set_coord_range: coord_range[0] and coord_range[1] - coord_range[0]
 
   // op helpers used by run()
   friend struct Net;

@@ -90,6 +90,34 @@ void nhwc_to_nchw(Ctx& cx, const TV& src, float* dst, int64_t dst_sn, int64_t ds
   parallel_for(cx, src.pixels() * src.c, NhwcToNchwK{src, dst, dst_sn, dst_sc, scale, shift, clamp01}, "nhwc_to_nchw");
 }
 
+// the same with sample n stored at row rows[n] of dst: up to kGatherMax rows per launch, carried in the kernel parameters
+struct NhwcToNchwRowsK {
+  NhwcToNchwK k; int rows[kGatherMax];
+  GV_HD void operator()(int64_t i) const {
+    const int64_t per = (int64_t)k.src.c * k.src.h * k.src.w;
+    const int n = (int)(i / per);
+    NhwcToNchwK s = k;
+    s.src.p = k.src.p + (int64_t)n * k.src.sn; s.src.n = 1;
+    s.dst = k.dst + (int64_t)rows[n] * k.sn;
+    s(i - n * per);
+  }
+};
+static void check_rows(const TV& src, const std::vector<int>& rows) {
+  if ((int)rows.size() != src.n) throw std::runtime_error("store_rows: one destination row per sample is required");
+  for (int r : rows) if (r < 0) throw std::runtime_error("store_rows: negative destination row");
+}
+void nhwc_to_nchw_rows(Ctx& cx, const TV& src, float* dst, const std::vector<int>& rows, int64_t dst_sn, int64_t dst_sc, float scale, float shift,
+                       int clamp01) {
+  check_rows(src, rows);
+  for (int n0 = 0; n0 < src.n; n0 += kGatherMax) {
+    const int cnt = std::min(src.n - n0, kGatherMax);
+    NhwcToNchwRowsK k{};
+    k.k = NhwcToNchwK{src.batch(n0, cnt), dst, dst_sn, dst_sc, scale, shift, clamp01};
+    for (int i = 0; i < cnt; ++i) k.rows[i] = rows[n0 + i];
+    parallel_for(cx, (int64_t)cnt * src.h * src.w * src.c, k, "nhwc_to_nchw_rows");
+  }
+}
+
 // The pointwise ops below with a 4-channel form are functor templates K<L, Any>: L channels per item, Any = half-aware storage
 // (precision mode 4's half tensors).  Each lane's arithmetic is written once; lanes_for picks the width.
 template <int L, bool Any> struct CopyK {
@@ -161,6 +189,32 @@ GV_HD float fv_div(float a, float b) {
   return a / b;
 #endif
 }
+// sample_coord_input (model.sample_coords, CoordSampler3D.shape2coordinate) of n samples at their own t, as (n, hc, wc, 3) (t, y, x),
+// and the (n) t vector.  The float32 arithmetic of torch on the device, one rounding per operation: a coordinate is
+// lo + span * ((i + 0.5) * (1 / size)) - true division by a host scalar is a product with its float reciprocal there.
+struct QueryCoordsK {
+  float* coords; float* tout; int hc, wc; float lo, span, ry, rx; float t[kGatherMax];
+  GV_HD void operator()(int64_t i) const {
+    const int x = (int)(i % wc); int64_t r = i / wc;
+    const int y = (int)(r % hc); const int n = (int)(r / hc);
+    float* o = coords + i * 3;
+    o[0] = t[n];
+    o[1] = fv_add(lo, fv_mul(span, fv_mul(fv_add((float)y, 0.5f), ry)));
+    o[2] = fv_add(lo, fv_mul(span, fv_mul(fv_add((float)x, 0.5f), rx)));
+    if (y == 0 && x == 0) tout[n] = t[n];
+  }
+};
+void query_coords(Ctx& cx, const std::vector<float>& t, int hc, int wc, float lo, float span, float* coords, float* tdev) {
+  for (size_t n0 = 0; n0 < t.size(); n0 += kGatherMax) {
+    const int cnt = (int)std::min(t.size() - n0, (size_t)kGatherMax);
+    QueryCoordsK k{};
+    k.coords = coords + (int64_t)n0 * hc * wc * 3; k.tout = tdev + n0; k.hc = hc; k.wc = wc; k.lo = lo; k.span = span;
+    k.ry = 1.0f / (float)hc; k.rx = 1.0f / (float)wc;
+    for (int i = 0; i < cnt; ++i) k.t[i] = t[n0 + i];
+    parallel_for(cx, (int64_t)cnt * hc * wc, k, "query_coords");
+  }
+}
+
 GV_HD float fv_sqrt(float a) {
 #ifdef __CUDA_ARCH__
   return __fsqrt_rn(a);
@@ -1466,6 +1520,28 @@ struct CombineOutK {
 };
 void combine_output(Ctx& cx, const TV& mean3, const TV& conv3, float* dst_nchw) {
   parallel_for(cx, mean3.pixels() * 3, CombineOutK{mean3, conv3, dst_nchw}, "combine_output");
+}
+// the same with sample n stored at image rows[n] of dst
+struct CombineOutRowsK {
+  CombineOutK k; int rows[kGatherMax];
+  GV_HD void operator()(int64_t i) const {
+    const int64_t per = (int64_t)3 * k.mean3.h * k.mean3.w;
+    const int n = (int)(i / per);
+    CombineOutK s = k;
+    s.mean3.p = k.mean3.p + (int64_t)n * k.mean3.sn; s.conv3.p = k.conv3.p + (int64_t)n * k.conv3.sn;
+    s.dst = k.dst + (int64_t)rows[n] * per;
+    s(i - n * per);
+  }
+};
+void combine_output_rows(Ctx& cx, const TV& mean3, const TV& conv3, float* dst_nchw, const std::vector<int>& rows) {
+  check_rows(mean3, rows);
+  for (int n0 = 0; n0 < mean3.n; n0 += kGatherMax) {
+    const int cnt = std::min(mean3.n - n0, kGatherMax);
+    CombineOutRowsK k{};
+    k.k = CombineOutK{mean3.batch(n0, cnt), conv3.batch(n0, cnt), dst_nchw};
+    for (int i = 0; i < cnt; ++i) k.rows[i] = rows[n0 + i];
+    parallel_for(cx, (int64_t)cnt * mean3.h * mean3.w * 3, k, "combine_output_rows");
+  }
 }
 
 // ---- LPIPS (AlexNet, v0.1; src/utils/lpips) ----

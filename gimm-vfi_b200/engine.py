@@ -7,7 +7,7 @@ from typing import Dict, Optional
 
 import torch
 
-from ._lib import IO, Clip, FlowInputs, Lib, Problem, View, default_lib
+from ._lib import IO, Clip, FlowInputs, Lib, Problem, Queries, View, default_lib
 
 
 # The auxiliary outputs of GIMMVFI_R / GIMMVFI_F.forward: key of the returned dict -> the engine outputs it is made of
@@ -331,6 +331,74 @@ class EngineHandle:
             c, flat = self._clip_struct(F, pl)
             self.lib.check(self.lib.dll.gimmvfi_forward_clip(self._h, C.byref(p), C.byref(c), C.byref(io), C.c_void_p(self._ws.data_ptr()),
                                                              self._ws.numel(), self._stream()), self._h)
+        return out
+
+    @staticmethod
+    def _queries_struct(n_frames: int, queries):
+        """a gimmvfi_queries and the host arrays it points at (keep all three alive for the call)"""
+        ql = [(int(a), int(b), float(t)) for a, b, t in queries]
+        flat = (C.c_int32 * max(2 * len(ql), 1))(*[i for a, b, _ in ql for i in (a, b)])
+        ts = (C.c_float * max(len(ql), 1))(*[t for _, _, t in ql])
+        return Queries(int(n_frames), len(ql), C.cast(flat, C.c_void_p), C.cast(ts, C.c_void_p)), flat, ts
+
+    @staticmethod
+    def query_pairs(queries):
+        """the distinct (src, tgt) pairs of a query list in first-appearance order, and each query's index among them"""
+        pairs, index = {}, []
+        for a, b, _ in queries:
+            index.append(pairs.setdefault((int(a), int(b)), len(pairs)))
+        return list(pairs), index
+
+    def queries_workspace_bytes(self, n_frames, queries, Hf, Wf, ds, Hc, Wc) -> int:
+        """workspace bytes of forward_queries with this frame count and query list.  The plan depends on the frame count, the distinct
+        pairs and their timestep counts only: plans are cached on that structure (the CLIP_PLANS most recent ones)."""
+        pairs, index = self.query_pairs(queries)
+        counts = tuple(index.count(i) for i in range(len(pairs)))
+        key = ("queries", int(n_frames), tuple(pairs), counts, Hf, Wf, float(ds) if ds else 0.0, Hc, Wc, self.weights_version)
+        if key in self._plans:
+            self._plans[key] = self._plans.pop(key)   # (most recently used last)
+        # any query list of this structure plans alike: t = 0.5 throughout
+        rep = [(a, b, 0.5) for (a, b), c in zip(pairs, counts) for _ in range(c)]
+        p = self._problem(len(pairs), Hf, Wf, max(counts), ds, Hc, Wc)
+        q, flat, ts = self._queries_struct(n_frames, rep)
+        n = self._plan(key, lambda nb: self.lib.dll.gimmvfi_plan_queries(self._h, C.byref(p), C.byref(q), nb))
+        qkeys = [k for k in self._plans if k[0] == "queries"]
+        for k in qkeys[:max(0, len(qkeys) - self.CLIP_PLANS)]:
+            del self._plans[k]
+        return n
+
+    def forward_queries(self, frames: torch.Tensor, queries, ds: Optional[float] = None, aux_outputs=True,
+                        coord_range=(-1.0, 1.0)) -> Dict[str, torch.Tensor]:
+        """A query list in one engine call (gimmvfi_forward_queries): frames (F,3,Hf,Wf) in [0,1] contiguous fp32 on self.device, queries
+        [(src, tgt, t), ...] with t strictly inside (0, 1).  The queries of one (src, tgt) are that pair's timesteps; the engine makes
+        the coordinates (sample_coord_input at the network resolution over coord_range) and t.  Returns the engine outputs: per-timestep
+        ones (Q, ...) in query order, raft_flow / nflow (P,2,2,H,W) over the distinct pairs in first-appearance order (query_pairs)."""
+        self._check_inputs(frames)
+        if frames.dim() != 4 or frames.shape[1] != 3:
+            raise ValueError("queries: frames must be (F,3,H,W), got %s" % (tuple(frames.shape),))
+        F, _, Hf, Wf = frames.shape
+        ql = [(int(a), int(b), float(t)) for a, b, t in queries]
+        if not ql:
+            raise ValueError("queries: at least one query is required")
+        Q = len(ql)
+        P = len(self.query_pairs(ql)[0])
+        H, W = (Hf, Wf) if not ds else (int(Hf * ds), int(Wf * ds))
+        aux = self._engine_aux(aux_outputs)
+        with self._guard():
+            self._workspace(self.queries_workspace_bytes(F, ql, Hf, Wf, ds, H, W))
+            E = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)
+            shapes = self._output_shapes(P, Hf, Wf, 1, H, W, H, W)
+            out = {"imgt_pred": E(Q, 3, Hf, Wf)}
+            out.update({f: E(*shapes[f]) if f in ("raft_flow", "nflow") else E(Q, *shapes[f][2:]) for f in aux})
+            io = IO()
+            io.img_xs = frames.data_ptr()
+            for k, v in out.items():
+                setattr(io, k, v.data_ptr())
+            p = self._problem(P, Hf, Wf, 1, ds, H, W)
+            q, flat, ts = self._queries_struct(F, ql)
+            self.lib.check(self.lib.dll.gimmvfi_set_coord_range(self._h, float(coord_range[0]), float(coord_range[1])), self._h)
+            self.lib.check(self.lib.dll.gimmvfi_forward_queries(self._h, C.byref(p), C.byref(q), C.byref(io), C.c_void_p(self._ws.data_ptr()),
+                                                                self._ws.numel(), self._stream()), self._h)
         return out
 
     def _launch(self, out, img_xs, coords, t, B, Hf, Wf, T, ds, Hc, Wc, frame_cache, flow_inputs):

@@ -4,6 +4,7 @@ gimmvfi_r.py:34-507).  Same constructor argument (``config.arch`` node), same
 414-key ``state_dict`` — but ``forward`` is one call into the sm_90a engine through
 the C ABI.  CUDA only; there is no PyTorch / CPU fallback path.
 """
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -164,6 +165,55 @@ class _VFIBase(_GIMMBase):
         o = eng.forward_clip(x, pl, coords.to(torch.float32).contiguous(), tt, ds_factor,
                              aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]])
         return model_outputs(o, len(ts), keys)
+
+    @staticmethod
+    def _check_query_args(frames, queries):
+        """interpolate_at's arguments -> [(src, tgt, t)] as (int, int, float); raises ValueError before any engine work"""
+        if not torch.is_tensor(frames) or frames.dim() != 4 or frames.shape[1] != 3 or frames.shape[0] < 1:
+            raise ValueError("interpolate_at: frames must be a (F,3,H,W) tensor with F >= 1, got %s"
+                             % (tuple(frames.shape) if torch.is_tensor(frames) else type(frames).__name__,))
+        F = frames.shape[0]
+        try:
+            ql = [(int(a), int(b), float(t)) for a, b, t in queries]
+        except (TypeError, ValueError):
+            raise ValueError("interpolate_at: queries must be a sequence of (source, target, t)")
+        if not ql:
+            raise ValueError("interpolate_at: the query list is empty")
+        bad = [q for q in ql if not (0 <= q[0] < F and 0 <= q[1] < F)]
+        if bad:
+            raise ValueError("interpolate_at: query(s) %s index outside the %d frames" % (bad, F))
+        # strictly inside (0, 1) as the float32 the engine receives: the AMT correlation lookup divides by t and 1 - t
+        # (gimmvfi_r.py:494-507); NaN fails both comparisons
+        with np.errstate(over="ignore"):
+            bad = [q for q in ql if not (0.0 < float(np.float32(q[2])) < 1.0)]
+        if bad:
+            raise ValueError("interpolate_at: query(s) %s have t outside the open interval (0, 1) in float32" % (bad,))
+        return ql
+
+    @torch.no_grad()
+    def interpolate_at(self, frames, queries, ds_factor=None):
+        """Every pair at its own timesteps, in one engine call: frames (F,3,H,W) in [0,1], queries [(src, tgt, t), ...] with t strictly
+        inside (0, 1).  The queries of one (src, tgt) are that pair's timesteps, in query order; each used frame is encoded once, and each
+        distinct pair's estimator runs once.  Query q's result is forward() with B = 1 on (frames[src], frames[tgt]) at its pair's own
+        timestep list, the coordinates sample_coord_input's at the network resolution.  Returns a dict keyed by engine output name:
+        imgt_pred (Q,3,H,W) and the outputs the aux_outputs selection maps to (AUX_OUTPUTS), per-timestep ones with the query axis first,
+        raft_flow / nflow (P,2,2,h,w) over the distinct pairs; plus pairs (the P distinct (src, tgt) in first-appearance order) and
+        pair_index (Q,), each query's index among them."""
+        return self._interpolate_at(frames, queries, ds_factor, self.aux_outputs)
+
+    def _interpolate_at(self, frames, queries, ds_factor, aux):
+        """interpolate_at's body; aux: an aux_outputs selection"""
+        ql = self._check_query_args(frames, queries)
+        if getattr(self, "flow_backend", None) is not None:
+            raise NotImplementedError("interpolate_at runs the engine's own flow estimator; model.flow_backend is only used by forward()")
+        eng = self._ready(frames)
+        x = frames.to(torch.float32).contiguous()
+        keys = aux_keys(aux)
+        out = eng.forward_queries(x, ql, ds_factor, aux_outputs=[f for k in keys for f in AUX_OUTPUTS[k]], coord_range=self.coord_range)
+        pairs, index = eng.query_pairs(ql)
+        out["pairs"] = pairs
+        out["pair_index"] = torch.tensor(index, dtype=torch.int64)
+        return out
 
     def compute_psnr(self, preds, targets, reduction="mean"):
         """gimmvfi_r.py:412-426 (the same in gimmvfi_f.py)"""

@@ -3,8 +3,10 @@ row 2.  uint8 frames go to the device once; /255, replicate-padding to a multipl
 src/utils/utils.py:156-185), the N-1 interpolations, un-padding and the uint8 (BGR) conversion all happen on
 the GPU; only uint8 frames cross the PCIe bus."""
 import ctypes as C
+from fractions import Fraction
 from typing import List, Optional
 
+import numpy as np
 import torch
 
 from ._lib import GimmvfiError, default_lib
@@ -182,3 +184,92 @@ class VideoInterpolator:
         self._prev = cur
         frames = [self._padder.unpad_u8(im, self.bgr)[0] for im in out["imgt_pred"]]
         return (frames, flow_images(self._padder, out["flowt"], self.bgr)) if self.with_flow else frames
+
+
+def _rate(x, name: str) -> Fraction:
+    """a frame rate as an exact rational: an int, a Fraction, or a string such as "30000/1001" or "29.97" (floats via their repr)"""
+    if isinstance(x, bool) or not isinstance(x, (int, float, str, Fraction)):
+        raise ValueError("%s must be an int, a Fraction or a string such as '30000/1001', got %r" % (name, x))
+    try:
+        r = Fraction(repr(x) if isinstance(x, float) else x.strip() if isinstance(x, str) else x)
+    except (ValueError, ZeroDivisionError):
+        raise ValueError("%s: cannot read %r as a frame rate" % (name, x))
+    if r <= 0:
+        raise ValueError("%s must be positive, got %s" % (name, r))
+    return r
+
+
+SNAP = Fraction(1, 10 ** 6)   # output instants this close to an input frame (in input frames) are that frame
+
+
+class FrameRateConverter:
+    """Frame-rate conversion of a clip streamed frame by frame: push() the (h,w,3) uint8 RGB input frames, get the output frames at
+    fps_out.  Output frame k shows input time tau_k = k * fps_in / fps_out (in input frames, exact rationals: no drift), for every k with
+    tau_k <= the last input frame.  A tau_k within SNAP (1e-6 input frames) of an input frame is that frame itself (no engine work; its
+    bytes, BGR-flipped when `bgr`); any other is the query (floor(tau), floor(tau) + 1, float32(tau - floor(tau))) of
+    GIMMVFI_R / GIMMVFI_F.interpolate_at, whose t then lies strictly inside (0, 1).  The tolerance matters for rates given as decimal
+    approximations, e.g. 30000/1001 as the float 29.97002997002997 that video readers report: their instants land a hair off the
+    input frames, where float32(t) rounds to 0 or 1 or the lookup's 1/t scaling is ill-conditioned; and no picture a hair away from
+    an input frame differs from it.  The converter keeps its own copy of the last frame pushed, so a caller may reuse its buffer.
+    Up to pairs_per_call K pairs that have queries go into one call, each frame encoded once; pairs without a query (60 -> 24 has
+    them) are never sent, and equal rates make no engine call at all.  Frames come back in output order: push() returns those that are
+    complete, flush() the rest at the end of a clip.  Pre- and post-processing are VideoInterpolator's (InputPadder, GPU uint8).
+    A call's workspace grows with K (model.engine.queries_workspace_bytes): at 1080p GIMM-VFI-R fits K = 4 for 24 -> 60 on an 80 GB
+    device but only K = 1 for 60 -> 24, whose pairs do not share frames (DESIGN §7)."""
+
+    def __init__(self, model, fps_in, fps_out, ds_factor: Optional[float] = None, bgr: bool = True, pairs_per_call: int = 1):
+        if isinstance(pairs_per_call, bool) or int(pairs_per_call) < 1:
+            raise ValueError("pairs_per_call must be >= 1, got %r" % (pairs_per_call,))
+        self.model, self.ds, self.bgr, self.pairs_per_call = model, ds_factor, bgr, int(pairs_per_call)
+        self.fps_in, self.fps_out = _rate(fps_in, "fps_in"), _rate(fps_out, "fps_out")
+        self.step = self.fps_in / self.fps_out   # input frames per output frame
+        self._padder = None
+        self.reset()
+
+    def reset(self):
+        """start a new clip: the next frame pushed is input frame 0"""
+        self._n = 0             # input frames pushed
+        self._k = 0             # next output index to schedule
+        self._prev_u8 = None    # a copy of the last frame pushed
+        self._queue = []        # scheduled outputs, in order: ("frame", uint8 (h,w,3)) or ("query", src, tgt, t)
+        self._frames = {}       # input index -> padded float frame (3,H,W), for the queries waiting
+
+    @torch.no_grad()
+    def flush(self) -> List[torch.Tensor]:
+        """interpolate the queries waiting and return every scheduled output frame, in order"""
+        queries = [e[1:] for e in self._queue if e[0] == "query"]
+        preds = iter(())
+        if queries:
+            used = sorted(self._frames)
+            local = {f: i for i, f in enumerate(used)}
+            frames = torch.stack([self._frames[f] for f in used], 0)
+            out = self.model._interpolate_at(frames, [(local[a], local[b], t) for a, b, t in queries], self.ds, False)
+            preds = iter(self._padder.unpad_u8(out["imgt_pred"], self.bgr).unbind(0))
+        res = [e[1] if e[0] == "frame" else next(preds) for e in self._queue]
+        self._queue, self._frames = [], {}
+        return res
+
+    @torch.no_grad()
+    def push(self, frame_u8: torch.Tensor) -> List[torch.Tensor]:
+        """the next input frame, (h,w,3) uint8 RGB -> the output frames completed by it, in order (uint8 (h,w,3), BGR when `bgr`)"""
+        if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
+            if self._queue:
+                raise ValueError("FrameRateConverter: the frame size changed with frames still waiting; flush() first")
+            self._padder = InputPadder(frame_u8.shape[:2], 32)
+            self.reset()
+        j = self._n
+        self._n += 1
+        while self._k * self.step <= j:   # the output instants in (j - 1, j] (frame 0: the instant 0)
+            off = self._k * self.step - (j - 1)   # in (0, 1]
+            self._k += 1
+            if off >= 1 - SNAP or off <= SNAP:    # input frame j, or (a hair after it) frame j - 1
+                u8 = frame_u8 if off >= 1 - SNAP else self._prev_u8
+                self._queue.append(("frame", u8.flip(-1) if self.bgr else u8.clone()))
+                continue
+            for f, u8 in ((j - 1, self._prev_u8), (j, frame_u8)):
+                if f not in self._frames:
+                    self._frames[f] = self._padder.pad_u8(u8.unsqueeze(0))[0]
+            self._queue.append(("query", j - 1, j, float(np.float32(float(off)))))
+        self._prev_u8 = frame_u8.clone()
+        waiting = {(e[1], e[2]) for e in self._queue if e[0] == "query"}
+        return self.flush() if not waiting or len(waiting) >= self.pairs_per_call else []

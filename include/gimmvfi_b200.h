@@ -98,6 +98,34 @@ typedef struct gimmvfi_clip {
 int gimmvfi_plan_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, size_t* workspace_bytes);
 int gimmvfi_forward_clip(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_clip* clip, const gimmvfi_io* io, void* workspace,
                          size_t workspace_bytes, void* cuda_stream);
+/* ---- A query list in one call: every pair at its own timesteps (GIMM-VFI-R and GIMM-VFI-F with their own estimator) ----
+ * `frames` frames and `queries` queries (source, target, t).  The queries that share (source, target) are the timesteps of one pair, in
+ * query order; any pairs are allowed, as in the clip call.  Per used frame: the clip's per-frame stages (frames no query references are
+ * not read); per distinct pair: correlation, the estimator, GIMM's encoder and the decoders' feature upsampling, once; per query: one
+ * timestep of GIMM's decoder and the synthesis.  Query q's outputs are gimmvfi_forward's with batch 1 on (frame src, frame tgt) at that
+ * pair's own timestep list, with the splat's float-atomic summation order as the only difference behind it: the same estimator path,
+ * and the same choice of GIMM's correlation lookup (volume-free for a pair of at most 2 timesteps, the all-pairs pyramid otherwise).
+ * Every index must lie in [0, frames) and every t strictly inside (0, 1) (the lookup divides by t and 1 - t); anything else fails
+ * before a launch.
+ * problem supplies height, width, ds_factor, coord_height and coord_width; its batch and timesteps are ignored.  The engine makes each
+ * query's coordinate grid (sample_coord_input at the network resolution, over the range of gimmvfi_set_coord_range) and t on the
+ * device: io->coords and io->t must be NULL.  io->img_xs points at the frames, (F,3,Hf,Wf) in [0,1].  Per-timestep outputs are (Q,...)
+ * in query order in place of (T,B,...); raft_flow and nflow are (P,2,2,H,W) over the P distinct pairs in first-appearance order.
+ * gimmvfi_plan_queries reports the workspace; it depends on the frame count, the distinct pair list and each pair's timestep count,
+ * not on the t values, so a retimer whose pattern of pairs and counts repeats reuses one plan.  Not recorded as a CUDA graph; the
+ * frame cache does not apply. */
+typedef struct gimmvfi_queries {
+  int32_t frames;              /* F >= 1                                      */
+  int32_t queries;             /* Q >= 1                                      */
+  const int32_t* pair_list;    /* HOST (Q,2): source, target frame index     */
+  const float* t;              /* HOST (Q): the timestep of each query        */
+} gimmvfi_queries;
+int gimmvfi_plan_queries(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_queries* queries, size_t* workspace_bytes);
+int gimmvfi_forward_queries(gimmvfi_engine* e, const gimmvfi_problem* p, const gimmvfi_queries* queries, const gimmvfi_io* io,
+                            void* workspace, size_t workspace_bytes, void* cuda_stream);
+/* The model's coord_range [lo, hi] for the query grids (default [-1, 1]): coordinate = lo + (hi - lo) * c in float32, (hi - lo) taken
+ * in double first, as sample_coord_input computes it. */
+int gimmvfi_set_coord_range(gimmvfi_engine* e, double lo, double hi);
 
 /* ---- GIMM-VFI-F (gimmvfi_f.py): everything downstream of the flow estimator ----
  * GIMMVFI_F.forward = FlowFormer (cal_bidirection_flow, gimmvfi_f.py:114-138) + exactly the GIMM / synthesis stages of GIMM-VFI-R
