@@ -435,7 +435,8 @@ void alt_corr_backward(Ctx& cx, const AltCorrArgs& a, const float* corr_grad, fl
 // ops_pointwise.cu
 void nchw_to_nhwc(Ctx& cx, const float* src, int64_t src_sn, int64_t src_sc, const TV& dst, float scale, float shift);
 void nhwc_to_nchw(Ctx& cx, const TV& src, float* dst, int64_t dst_sn, int64_t dst_sc, float scale, float shift, int clamp01);  // (v + shift) * scale
-// index-table stores: sample n of src goes to row rows[n] of dst (rows ride in the kernel parameters, kGatherMax per launch)
+// index-table stores: sample n of src goes to row rows[n] of dst (rows ride in the kernel parameters, kGatherMax per launch;
+// consecutive rows take the plain store)
 constexpr int kGatherMax = 64;
 void nhwc_to_nchw_rows(Ctx& cx, const TV& src, float* dst, const std::vector<int>& rows, int64_t dst_sn, int64_t dst_sc, float scale, float shift,
                        int clamp01);

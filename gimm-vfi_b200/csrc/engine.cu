@@ -1007,6 +1007,11 @@ static void gather_samples(Ctx& cx, const TV& src, const std::vector<int>& idx, 
   else gather_samples_as<uint32_t>(cx, src, idx, dst, bytes);
 }
 
+static bool is_identity(const std::vector<int>& idx) {
+  for (size_t i = 0; i < idx.size(); ++i) if (idx[i] != (int)i) return false;
+  return true;
+}
+
 static void check_problem(const Problem& p) {
   if (p.B < 1 || p.T < 1) throw std::runtime_error("gimmvfi: B and T must be >= 1");
   const int H = p.H(), W = p.W();
@@ -1016,20 +1021,57 @@ static void check_problem(const Problem& p) {
     throw std::runtime_error("gimmvfi: coordinate grid must match the network resolution (frame_synthesize consumes flow_t at that size)");
 }
 
-// A query list as run() takes it.  The distinct pairs are ordered by timestep count, descending (stable), so that timestep slot k runs
-// over the prefix of the pairs that have more than k timesteps: every per-pair buffer is batch-major, and slot k works on .batch(0, B_k)
-// views.  Only the frames some query uses are read and encoded.
-struct QuerySchedule {
-  std::vector<int> frames;           // the used frames, ascending: compact frame i is caller frame frames[i]
-  Clip clip;                         // over the compact frames, pairs in slot order
-  std::vector<int> first;            // pair i's row among the distinct pairs in first-appearance order (raft_flow, nflow)
-  std::vector<std::vector<int>> q;   // pair i's queries, in query order: slot k's output row of pair i is q[i][k]
-  std::vector<float> t;              // (Q) the t of every query
-  int T = 0;                         // slots: the largest timestep count
-  int slot_pairs(int k) const { int n = 0; while (n < (int)q.size() && (int)q[n].size() > k) ++n; return n; }
+// What run() interpolates: the caller frames it reads, the pairs of them, and the output rows of each timestep slot.  The pairs are
+// ordered by timestep count, descending, so that slot k runs over the B_k pairs that have more than k timesteps, a prefix: every
+// per-pair buffer is batch-major, and slot k works on .batch(0, B_k) views.  One builder per input form validates it and fills this in.
+struct Schedule {
+  struct Load { int64_t off, sn, sc; int f0, n; };   // io.img_xs + off, sample / channel strides sn / sc -> engine frames [f0, f0 + n)
+  std::vector<Load> loads;
+  int F = 0;                          // engine frames
+  std::vector<int> src, tgt;          // pair p interpolates from engine frame src[p] to tgt[p]
+  std::vector<int> pair_rows;         // pair p's row of raft_flow / nflow
+  std::vector<std::vector<int>> rows; // slot k: the output row of each of its B_k pairs
+  std::vector<float> t;               // the t of every output row; empty: io.t / io.coords at the slot's rows (then consecutive)
+  int per_call = 1;                   // FlowFormer: pairs per reference call
+  int decide_as = 2;                  // RAFT: choose the lookup path as a run of this many pairs would (0: the pair count)
+  bool frame_cache = false;           // the R frame cache (set_frame_cache) may be used
 };
 
-static QuerySchedule schedule_queries(const Queries& qs) {
+// forward_clip(): the F frames of a (F,3,Hf,Wf) input and P = B pairs of them, T timesteps each.  Pair p takes the paths of forward() with
+// B = 1 on its frames: one FlowFormer call per direction, and RAFT's lookup chosen for 2 directions (the clip's workspace holds 2P volumes).
+static Schedule schedule_clip(const Problem& p, const Clip& c) {
+  check_problem(p);
+  if ((int)c.src.size() != p.B || (int)c.tgt.size() != p.B) throw std::runtime_error("gimmvfi clip: problem batch must equal the number of pairs");
+  for (int i = 0; i < p.B; ++i)
+    if (c.src[i] < 0 || c.src[i] >= c.F || c.tgt[i] < 0 || c.tgt[i] >= c.F)
+      throw std::runtime_error("gimmvfi clip: pair " + std::to_string(i) + " = (" + std::to_string(c.src[i]) + ", " + std::to_string(c.tgt[i]) +
+                               ") indexes outside the " + std::to_string(c.F) + " frames");
+  Schedule s;
+  s.loads = {{0, 3 * (int64_t)p.Hf * p.Wf, (int64_t)p.Hf * p.Wf, 0, c.F}};
+  s.F = c.F; s.src = c.src; s.tgt = c.tgt;
+  s.rows.resize(p.T);
+  for (int b = 0; b < p.B; ++b) {
+    s.pair_rows.push_back(b);
+    for (int k = 0; k < p.T; ++k) s.rows[k].push_back(k * p.B + b);
+  }
+  return s;
+}
+
+// forward(): a clip of the frame stack [I0 batch ; I1 batch] of a (B,3,2,Hf,Wf) input and its B pairs (b, B + b), which the estimators
+// run batched, and the only form the frame cache serves
+static Schedule schedule_batch(const Problem& p) {
+  Clip c; c.F = 2 * p.B;
+  for (int b = 0; b < p.B; ++b) { c.src.push_back(b); c.tgt.push_back(p.B + b); }
+  Schedule s = schedule_clip(p, c);
+  const int64_t hw = (int64_t)p.Hf * p.Wf;
+  s.loads = {{0, 6 * hw, 2 * hw, 0, p.B}, {hw, 6 * hw, 2 * hw, p.B, p.B}};
+  s.per_call = p.B; s.decide_as = 0; s.frame_cache = true;
+  return s;
+}
+
+// forward_queries(): the queries' distinct pairs, their timesteps in query order and the per-query t.  Only the frames some query uses are
+// read and encoded.  The problem's B and T are those of the list.
+static Schedule schedule_queries(const Problem& p, const Queries& qs) {
   const int Q = (int)qs.src.size(), F = qs.F;
   if (Q < 1) throw std::runtime_error("gimmvfi queries: at least one query is required");
   if (F < 1) throw std::runtime_error("gimmvfi queries: at least one frame is required");
@@ -1052,17 +1094,25 @@ static QuerySchedule schedule_queries(const Queries& qs) {
   std::vector<int> order(pairs.size());
   for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
   std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return q[x].size() > q[y].size(); });
-  QuerySchedule s;
-  std::vector<int> compact(F, -1);
+  Problem e = p; e.B = (int)pairs.size(); e.T = (int)q[order[0]].size();
+  check_problem(e);
+  Schedule s;
+  std::vector<int> compact(F, -1);   // the engine frame of each used caller frame, in caller order
   for (const auto& ab : pairs) compact[ab.first] = compact[ab.second] = 0;
-  for (int f = 0; f < F; ++f) if (compact[f] == 0) { compact[f] = (int)s.frames.size(); s.frames.push_back(f); }
-  s.clip.F = (int)s.frames.size();
+  const int64_t hw = (int64_t)p.Hf * p.Wf;
+  for (int f = 0; f < F; ++f) {
+    if (compact[f] < 0) continue;
+    if (f > 0 && compact[f - 1] >= 0) ++s.loads.back().n;   // one load per run of consecutive used frames
+    else s.loads.push_back({f * 3 * hw, 3 * hw, hw, s.F, 1});
+    compact[f] = s.F++;
+  }
+  s.rows.resize(e.T);
   for (int d : order) {
-    s.clip.src.push_back(compact[pairs[d].first]); s.clip.tgt.push_back(compact[pairs[d].second]);
-    s.first.push_back(d); s.q.push_back(q[d]);
+    s.src.push_back(compact[pairs[d].first]); s.tgt.push_back(compact[pairs[d].second]);
+    s.pair_rows.push_back(d);
+    for (size_t k = 0; k < q[d].size(); ++k) s.rows[k].push_back(q[d][k]);
   }
   s.t = qs.t;
-  s.T = (int)s.q[0].size();
   return s;
 }
 
@@ -1081,8 +1131,7 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   std::vector<int> srcs, slot(F, -1);   // distinct sources in first-use order
   for (int s = 0; s < S; ++s)
     if (slot[src[s]] < 0) { slot[src[s]] = (int)srcs.size(); srcs.push_back(src[s]); }
-  bool in_order = !r.gather && S == F;
-  for (int s = 0; in_order && s < S; ++s) in_order = src[s] == s;
+  const bool in_order = !r.gather && S == F && is_identity(src);
   if (r.enc0 && !in_order) throw std::runtime_error("raft: skipping encoders needs the sources in frame order");
   const int ns = (int)srcs.size(), e0 = r.enc0, en = F - e0;
   TV hx = A.tensor(S, h, w, 384);                      // [h | inp | motion]
@@ -1232,10 +1281,28 @@ void Engine::run_raft(Ctx& cx, Net& N, const RaftRun& r) {
   tap("raft.net_final", hcur);
 }
 
-void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin, const Clip* clip, const QuerySchedule* qs) {
+// The frame cache (set_frame_cache) of a batch forward, between RAFT's encoders and its GRU (which overwrites net in place): with
+// `load` frame 0's products come from the cache, with `store` frame 1's are written to it.  ni: the pairs' net | inp.
+void Engine::frame_cache(Ctx& cx, const Problem& P, const TV& fmap, const TV& ni, const TV& feat4, const TV& feat8) {
+  const int B = P.B, H = P.H(), W = P.W();
+  if (fc_bytes_ < frame_cache_bytes(P)) throw std::runtime_error("gimmvfi: frame cache smaller than frame_cache_bytes()");
+  const auto fc_it = fc_valid_.find(fc_);
+  if (fc_load_ && (fc_it == fc_valid_.end() || fc_it->second.B != B || fc_it->second.H != H || fc_it->second.W != W || fc_it->second.mode != tc_mode_))
+    throw std::runtime_error("gimmvfi: frame cache load requested, but this buffer does not hold a frame stored by a forward of the same "
+                             "problem size and precision mode");
+  if (fc_store_) fc_valid_[fc_] = FcRec{B, H, W, tc_mode_};
+  else if (!fc_load_) fc_valid_.erase(fc_);
+  float* q = fc_;
+  for (const TV& t : {fmap, ni, feat4, feat8}) {   // the cache: B dense samples of each, in this order
+    const TV c = make_tv(q, B, t.h, t.w, t.c); q += (size_t)B * t.h * t.w * t.c;
+    if (fc_load_) copy_channels(cx, c, t.batch(0, B));
+    if (fc_store_) copy_channels(cx, t.batch(B, B), c);
+  }
+}
+
+void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const Schedule& sched, const FlowInputs* fin) {
   Problem P = P0;
-  if (qs) { clip = &qs->clip; P.B = (int)qs->clip.src.size(); P.T = qs->T; }   // a query list: its distinct pairs and slots
-  check_problem(P);
+  P.B = (int)sched.src.size(); P.T = (int)sched.rows.size();   // (a query list's distinct pairs and slots; the problem's own otherwise)
   Net N{*this, cx};
   Arena& A = cx.arena;
   const int B = P.B, Hf = P.Hf, Wf = P.Wf, H = P.H(), W = P.W(), T = P.T;
@@ -1246,69 +1313,53 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
   const float inv = (float)inv_d, rinv = (float)(1.0 / inv_d);
 
   // The estimator's pair list over the frame stack: both directions of every pair, [pairs ; reversed pairs], which is also the sample
-  // order of everything downstream.  A batch forward's frames are [I0 batch ; I1 batch]; a clip's are its own F frames, and the
-  // per-frame products they make are gathered into pair order (fslot: a frame's sample among the distinct sources, first-use order).
-  const int NF = clip ? clip->F : 2 * B;
-  std::vector<int> esrc(2 * B), etgt(2 * B), fslot(NF, -1);
+  // order of everything downstream.  The per-frame products are gathered into that order unless it is the frames' own (a batch
+  // forward's [I0 batch ; I1 batch]); fslot: a frame's sample among the distinct sources, first-use order.
+  std::vector<int> esrc(2 * B), etgt(2 * B), pslot(2 * B), fslot(sched.F, -1);   // pslot: each sample's distinct-source slot
+  for (int s = 0; s < B; ++s) { esrc[s] = etgt[B + s] = sched.src[s]; etgt[s] = esrc[B + s] = sched.tgt[s]; }
   int nsrc = 0;
-  if (clip) {
-    if (fin) throw std::runtime_error("gimmvfi: a clip runs the engine's own flow estimator");
-    if (clip->F < 1 || (int)clip->src.size() != B || (int)clip->tgt.size() != B) throw std::runtime_error("gimmvfi: bad clip (frames or pair count)");
-    for (int s = 0; s < B; ++s) {
-      if (clip->src[s] < 0 || clip->src[s] >= NF || clip->tgt[s] < 0 || clip->tgt[s] >= NF)
-        throw std::runtime_error("gimmvfi: clip pair " + std::to_string(s) + " indexes outside the " + std::to_string(NF) + " frames");
-      esrc[s] = etgt[B + s] = clip->src[s]; etgt[s] = esrc[B + s] = clip->tgt[s];
-    }
-  } else {
-    for (int s = 0; s < 2 * B; ++s) { esrc[s] = s; etgt[s] = s < B ? s + B : s - B; }
-  }
-  for (int s : esrc) if (fslot[s] < 0) fslot[s] = nsrc++;
-  std::vector<int> pslot(2 * B);   // each sample's distinct-source slot
-  for (int s = 0; s < 2 * B; ++s) pslot[s] = fslot[esrc[s]];
+  for (int s = 0; s < 2 * B; ++s) { if (fslot[esrc[s]] < 0) fslot[esrc[s]] = nsrc++; pslot[s] = fslot[esrc[s]]; }
+  // x's samples in pair order, sample i <- x's sample idx[i]: x itself when idx is the identity, else gathered into `into` (or a new tensor)
+  auto pair_order = [&](const TV& x, const std::vector<int>& idx, TV into = TV()) {
+    if (is_identity(idx)) return x;
+    if (!into.p) into = x.f16 ? A.tensor_h((int)idx.size(), x.h, x.w, x.c, x.ld) : A.tensor((int)idx.size(), x.h, x.w, x.c, x.ld);
+    gather_samples(cx, x, idx, into);
+    return into;
+  };
 
   // ------------------------------------------------------------ inputs
-  // frames as NHWC, stacked [I0 batch ; I1 batch] (a clip: its frames in order; a query list: its used frames, in runs of consecutive ones)
-  TV full01 = A.tensor(NF, Hf, Wf, 3, 4);
-  if (qs)
-    for (int i0 = 0, i1; i0 < NF; i0 = i1) {
-      for (i1 = i0 + 1; i1 < NF && qs->frames[i1] == qs->frames[i1 - 1] + 1;) ++i1;
-      nchw_to_nhwc(cx, io.img_xs + (int64_t)qs->frames[i0] * 3 * Hf * Wf, (int64_t)3 * Hf * Wf, (int64_t)Hf * Wf, full01.batch(i0, i1 - i0), 1.f, 0.f);
-    }
-  else if (clip)
-    nchw_to_nhwc(cx, io.img_xs, (int64_t)3 * Hf * Wf, (int64_t)Hf * Wf, full01, 1.f, 0.f);
-  else
-    for (int f = 0; f < 2; ++f)
-      nchw_to_nhwc(cx, io.img_xs + (int64_t)f * Hf * Wf, (int64_t)6 * Hf * Wf, (int64_t)2 * Hf * Wf, full01.batch(f * B, B), 1.f, 0.f);
+  TV full01 = A.tensor(sched.F, Hf, Wf, 3, 4);   // frames as NHWC
+  for (const Schedule::Load& l : sched.loads) nchw_to_nhwc(cx, io.img_xs + l.off, l.sn, l.sc, full01.batch(l.f0, l.n), 1.f, 0.f);
   TV img01 = full01;
   if (ds) {
-    img01 = A.tensor(NF, H, W, 3, 4);
+    img01 = A.tensor(sched.F, H, W, 3, 4);
     resize_bilinear(cx, full01, img01, rds, rds, 1.f, 0, ACT_NONE);  // gimmvfi_r.py:329-337
   }
-  TV raft_in = A.tensor(NF, H, W, 3, 4);
-  TV syn = A.tensor(NF, H, W, 3, 4);       // 2*x - 1  (gimmvfi_r.py:230-231)
+  TV raft_in = A.tensor(sched.F, H, W, 3, 4);
+  TV syn = A.tensor(sched.F, H, W, 3, 4);  // 2*x - 1  (gimmvfi_r.py:230-231)
   {
     // dense views (ld == 4): run over the padded buffers, padding lane included (harmless)
-    int64_t cnt = (int64_t)NF * H * W * 4;
+    int64_t cnt = (int64_t)sched.F * H * W * 4;
     TV s = img01; s.c = 4; TV d = raft_in; d.c = 4;
     parallel_for(cx, cnt, RaftPrepK{s, d}, "raft_prep");
     parallel_for(cx, cnt, ScaleShiftK{img01.p, syn.p, 2.f, 1.0f}, "img_to_pm1");
   }
   TV synf = syn;
   if (ds) {
-    synf = A.tensor(NF, Hf, Wf, 3, 4);
-    parallel_for(cx, (int64_t)NF * Hf * Wf * 4, ScaleShiftK{full01.p, synf.p, 2.f, 1.0f}, "img_to_pm1_full");
+    synf = A.tensor(sched.F, Hf, Wf, 3, 4);
+    parallel_for(cx, (int64_t)sched.F * Hf * Wf * 4, ScaleShiftK{full01.p, synf.p, 2.f, 1.0f}, "img_to_pm1_full");
   }
 
   // persistent across stages
   TV flow_up = A.tensor(2 * B, H, W, 2);            // [f01 ; f10]
-  TV fmap = A.tensor(NF, h, w, 256);                // fnet features of [I0 ; I1]
+  TV fmap = A.tensor(sched.F, h, w, 256);           // fnet features of every frame
   TV feat4 = A.tensor(nsrc, H4, W4, 128), feat8 = A.tensor(nsrc, h, w, 256);  // projected context features
   float* scaler = A.alloc_f(std::max(B, 64));
 
   // ------------------------------------------------------------ RAFT (both directions batched)
   // The recurrence amplifies operand rounding -> fp32-class arithmetic only: 3xTF32 tensor cores or CUDA cores.
   cx.tc = tc_mode_ >= 2; cx.tc_split = true;
-  TV fproj = A.tensor(NF, h, w, 256);               // the maps BidirCorrBlock correlates (R: amt_fproj(fnet map); F: the estimator's own)
+  TV fproj = A.tensor(sched.F, h, w, 256);          // the maps BidirCorrBlock correlates (R: amt_fproj(fnet map); F: the estimator's own)
   if (fin) {
     // external flow estimator (GIMM-VFI-F): NCHW -> the engine's NHWC buffers, samples [frame-0 batch ; frame-1 batch]
     for (int j = 0; j < 2; ++j) {
@@ -1319,56 +1370,31 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
     }
   } else if (is_f()) {
     // GIMM-VFI-F: the native FlowFormer estimator fills the same four products (gimmvfi_f.py:114-138); F has no feature projections.
-    // Frames [I0 ; I1]: pairs (b, B + b), then (B + b, b), one reference call per direction; a clip: one reference call per pair and
-    // direction, as a batch forward with B = 1 makes them
-    run_flowformer(cx, N, raft_in, esrc, etgt, clip ? 1 : B, ff_iters, false, flow_up, TV(), feat4, feat8, fproj);
+    // The schedule's pairs (b, B + b), then (B + b, b): a batch forward makes one reference call per direction, a clip or a query list
+    // one per pair and direction, as a batch forward with B = 1 makes them
+    run_flowformer(cx, N, raft_in, esrc, etgt, sched.per_call, ff_iters, false, flow_up, TV(), feat4, feat8, fproj);
   } else {
     const size_t mk = A.mark();
-    // frame cache (set_frame_cache): with `load` the encoders only see the second frames, samples [B, 2B).  Not for clips.
-    const bool fc_on = fc_ != nullptr && !cx.dry && !clip;
-    if (fc_on && fc_bytes_ < frame_cache_bytes(P)) throw std::runtime_error("gimmvfi: frame cache smaller than frame_cache_bytes()");
-    const bool fload = fc_on && fc_load_, fstore = fc_on && fc_store_;
-    const auto fc_it = fc_valid_.find(fc_);
-    if (fload && (fc_it == fc_valid_.end() || fc_it->second.B != B || fc_it->second.H != H || fc_it->second.W != W || fc_it->second.mode != tc_mode_))
-      throw std::runtime_error("gimmvfi: frame cache load requested, but this buffer does not hold a frame stored by a forward of the same "
-                               "problem size and precision mode");
-    const int e0 = fload ? B : 0, en = fload ? B : nsrc;
-    // both directions batched: frames [I0 ; I1], pairs (b, B + b) then (B + b, b) (gimmvfi_r.py:126-132).  c4 / c8 below are those
-    // of the distinct sources in first-use order, i.e. feat4 / feat8's slots.
+    // frame cache: with `load` the encoders only see the second frames, samples [B, 2B)
+    const bool fc_on = sched.frame_cache && fc_ != nullptr && !cx.dry;
+    const int e0 = fc_on && fc_load_ ? B : 0, en = nsrc - e0;
+    // both directions batched (gimmvfi_r.py:126-132); c4 / c8 below are the distinct sources', first-use order: feat4 / feat8's slots
     RaftRun r;
     r.img = raft_in; r.iters = raft_iters; r.flow_up = flow_up; r.fmap = fmap; r.enc0 = e0;
-    r.src = esrc; r.tgt = etgt;
-    if (clip) r.decide_as = 2;   // pair p takes the lookup path of forward() with B = 1 on its frames: the clip's workspace holds 2P volumes
+    r.src = esrc; r.tgt = etgt; r.decide_as = sched.decide_as;
     r.encoded = [&](const TV& c4, const TV& c8, const TV& hx) {
       // context features for the synthesis net (gimmvfi_r.py:134-141)
       N.conv("amt_second_last_cproj", c4, feat4.batch(e0, en));
       N.conv("amt_last_cproj", c8, feat8.batch(e0, en));
-      if (!fc_on) return;
-      float* q = fc_;
-      TV c_fmap = make_tv(q, B, h, w, 256); q += (size_t)B * h * w * 256;
-      TV c_ni = make_tv(q, B, h, w, 256); q += (size_t)B * h * w * 256;
-      TV c_f4 = make_tv(q, B, H4, W4, 128); q += (size_t)B * H4 * W4 * 128;
-      TV c_f8 = make_tv(q, B, h, w, 256);
-      if (fload) {
-        copy_channels(cx, c_fmap, fmap.batch(0, B)); copy_channels(cx, c_ni, hx.batch(0, B).slice(0, 256));
-        copy_channels(cx, c_f4, feat4.batch(0, B)); copy_channels(cx, c_f8, feat8.batch(0, B));
-      }
-      if (fstore) fc_valid_[fc_] = FcRec{B, H, W, tc_mode_};
-      else if (!fload) fc_valid_.erase(fc_);
-      if (fstore) {   // (before the GRU overwrites `net` in place)
-        copy_channels(cx, fmap.batch(B, B), c_fmap); copy_channels(cx, hx.batch(B, B).slice(0, 256), c_ni);
-        copy_channels(cx, feat4.batch(B, B), c_f4); copy_channels(cx, feat8.batch(B, B), c_f8);
-      }
+      if (fc_on) frame_cache(cx, P, fmap, hx.slice(0, 256), feat4, feat8);
     };
     run_raft(cx, N, r);
     if (!debug_) A.release(mk);
   }
-  // (B,2,2,H,W) per-pair outputs from [direction 0 ; direction 1] samples; a query list's rows are its distinct pairs in first-appearance order
+  // (P,2,2,H,W) per-pair outputs from [direction 0 ; direction 1] samples, pair p at row pair_rows[p]
   auto store_pairs = [&](const TV& both, float* dst) {
-    for (int j = 0; j < 2; ++j) {
-      if (qs) nhwc_to_nchw_rows(cx, both.batch(j * B, B), dst + (int64_t)j * H * W, qs->first, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
-      else nhwc_to_nchw(cx, both.batch(j * B, B), dst + (int64_t)j * H * W, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
-    }
+    for (int j = 0; j < 2; ++j)
+      nhwc_to_nchw_rows(cx, both.batch(j * B, B), dst + (int64_t)j * H * W, sched.pair_rows, (int64_t)4 * H * W, (int64_t)2 * H * W, 1.f, 0.f, 0);
   };
   if (io.raft_flow) store_pairs(flow_up, io.raft_flow);
 
@@ -1376,28 +1402,17 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
   cx.tc = tc_mode_ >= 1; cx.tc_split = false;
   // ------------------------------------------------------------ bidirectional volume on projected features
   if (!fin && !is_f()) N.conv("amt_fproj", fmap, fproj);
-  if (clip) {   // per frame -> pair order: [sources ; targets] of the pairs
-    TV g = A.tensor(2 * B, h, w, 256);
-    gather_samples(cx, fproj, esrc, g);
-    fproj = g;
-    TV s2 = A.tensor(2 * B, H, W, 3, 4);
-    gather_samples(cx, syn, esrc, s2);
-    TV f2 = s2;
-    if (ds) {
-      f2 = A.tensor(2 * B, Hf, Wf, 3, 4);
-      gather_samples(cx, synf, esrc, f2);
-    }
-    syn = s2; synf = f2;
-  }
+  fproj = pair_order(fproj, esrc);   // [sources ; targets] of the pairs
+  syn = pair_order(syn, esrc);
+  synf = ds ? pair_order(synf, esrc) : syn;
   // the bidirectional volume only feeds TF32 layers (AMT update blocks) -> plain TF32 is at their input precision
-  // Few interpolated frames per pair (T <= corr_direct_max_t): no volume at all - the lookup computes the dot products its window needs
-  // (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up T times.  A query list decides per pair, as that pair's
-  // own forward would: its pairs are sorted by timestep count, so the pyramid pairs are a prefix [0, Bp) and the direct ones [Bp, B).
+  // Few interpolated frames per pair (at most corr_direct_max_t timesteps): no volume at all - the lookup computes the dot products its
+  // window needs (corr.cu "volume-free lookup").  Otherwise the all-pairs pyramid, looked up at every timestep.  Each pair decides as its
+  // own forward would: the pairs are sorted by timestep count, so the pyramid pairs are a prefix [0, Bp) and the direct ones [Bp, B).
   Pyramid bpyr{}; CorrFeat bfeat{};
   constexpr int corr_direct_max_t = 2;
   const bool direct_ok = tc_mode_ >= 1 && fproj.c == 256 && h >= 16 && w >= 16;
-  int Bp = direct_ok && T <= corr_direct_max_t ? 0 : B;
-  if (qs && direct_ok) { Bp = 0; while (Bp < B && (int)qs->q[Bp].size() > corr_direct_max_t) ++Bp; }
+  const int Bp = !direct_ok ? B : T > corr_direct_max_t ? (int)sched.rows[corr_direct_max_t].size() : 0;
   const int Bd = B - Bp;
   if (Bd > 0) {
     // half features of the direct pairs' samples, [sources ; targets]: compact sample i < Bd is pair Bp + i's source, Bd + i its target
@@ -1431,10 +1446,11 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
   // ------------------------------------------------------------ hoisted (t-independent) decoder feature upsampling
   TV fup4 = A.tensor(2 * B, H4, W4, 128);   // NewInitDecoder.upsample   fi_components.py:234-244
   TV fup1 = half_chains(cx) ? A.tensor_h(2 * B, H, W, 64) : A.tensor(2 * B, H, W, 64);      // NewMultiFlowDecoder.upsample fi_components.py:284-295
-  // a clip upsamples each distinct source once, then gathers the results into pair order
+  // each distinct source is upsampled once: straight into fup4 / fup1 when they are the pairs' samples in order, else into buffers of
+  // their own, gathered into pair order below
   const size_t fup_mk = A.mark();
   TV fup4s = fup4, fup1s = fup1;
-  if (clip) { fup4s = A.tensor(nsrc, H4, W4, 128); fup1s = half_chains(cx) ? A.tensor_h(nsrc, H, W, 64) : A.tensor(nsrc, H, W, 64); }
+  if (!is_identity(pslot)) { fup4s = A.tensor(nsrc, H4, W4, 128); fup1s = half_chains(cx) ? A.tensor_h(nsrc, H, W, 64) : A.tensor(nsrc, H, W, 64); }
   {
     const size_t mk = A.mark();
     const std::string p = "amt_init_decoder.upsample.";
@@ -1459,11 +1475,9 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
     N.conv(p + "7", d, fup1s, ACT_RELU);
     A.release(mk);
   }
-  if (clip) {
-    gather_samples(cx, fup4s, pslot, fup4);
-    gather_samples(cx, fup1s, pslot, fup1);
-    if (!debug_) A.release(fup_mk);
-  }
+  pair_order(fup4s, pslot, fup4);
+  pair_order(fup1s, pslot, fup1);
+  if (!debug_) A.release(fup_mk);
   tap("syn.feat4", feat4); tap("syn.feat8", feat8); tap("syn.fup4", fup4); tap("syn.fproj", fproj);
   tap_copy(cx, "syn.fup1", fup1);   // (half in mode 4)
 
@@ -1481,39 +1495,35 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
   gimm_encode(N, nf, f01, f10, wts, X64);
 
   // ------------------------------------------------------------ per-timestep: GIMM decode + frame synthesis
-  // A query list's slot ti runs over its first Bk pairs (those with more than ti timesteps): every per-pair buffer below is batch-major,
-  // so the slot works on .batch(0, Bk) views of the first direction and .batch(B, Bk) of the second.  Its coordinates and t are made
-  // here, and its outputs are stored at the rows of its queries.
+  // Slot ti runs over the first Bk pairs (those with more than ti timesteps): every per-pair buffer below is batch-major, so the slot
+  // works on .batch(0, Bk) views of the first direction and .batch(B, Bk) of the second, and stores its outputs at its rows.
   TV grid_flow = A.tensor(B, h, w, 4);   // flow_4_lr = cat(fl0, fl1)
   const size_t t_mark = A.mark();
   for (int ti = 0; ti < T; ++ti) {
     A.release(t_mark);
     // debug taps of the per-timestep tensors are taken at the last timestep: nothing overwrites them after it
     const bool last = ti == T - 1;
-    const int Bk = qs ? qs->slot_pairs(ti) : B;
-    const float* tdev = io.t ? io.t + (int64_t)ti * B : nullptr;
-    const float* coords_t = io.coords ? io.coords + (int64_t)ti * B * P.Hc * P.Wc * 3 : nullptr;
-    std::vector<int> rows;   // a query list: the output row (query) of each of the slot's samples
-    if (qs) {
+    const std::vector<int>& rows = sched.rows[ti];
+    const int Bk = (int)rows.size();
+    const float *tdev, *coords_t;
+    if (sched.t.empty()) {   // the caller's, at the slot's (consecutive) rows
+      tdev = io.t + rows[0];
+      coords_t = io.coords + (int64_t)rows[0] * P.Hc * P.Wc * 3;
+    } else {
       std::vector<float> ts;
-      for (int b = 0; b < Bk; ++b) { rows.push_back(qs->q[b][ti]); ts.push_back(qs->t[qs->q[b][ti]]); }
+      for (int r : rows) ts.push_back(sched.t[r]);
       float* tq = A.alloc_f(std::max(Bk, 64));
       float* cq = A.alloc_f((size_t)Bk * P.Hc * P.Wc * 3);
       if (!cx.dry) query_coords(cx, ts, P.Hc, P.Wc, coord_lo_, coord_span_, cq, tq);
       tdev = tq; coords_t = cq;
       if (last) tap("query.coords", make_tv(cq, Bk, P.Hc, P.Wc, 3));
     }
-    // per-timestep outputs (ti, B, ...): rows ti * B + b; a query list's: the rows of its queries
-    auto store = [&](const TV& src, float* dst, int64_t sn, int64_t sc, float scale, float shift, int clamp01) {
-      if (qs) nhwc_to_nchw_rows(cx, src, dst, rows, sn, sc, scale, shift, clamp01);
-      else nhwc_to_nchw(cx, src, dst + (int64_t)ti * B * sn, sn, sc, scale, shift, clamp01);
-    };
     TV ninr = A.tensor(Bk, H, W, 2);
     gimm_decode(N, X64.batch(0, Bk), f01.batch(0, Bk), f10.batch(0, Bk), wts.batch(0, Bk), wts.batch(B, Bk), tdev, coords_t, ninr, last);
-    if (io.ninrflow) store(ninr, io.ninrflow, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
+    if (io.ninrflow) nhwc_to_nchw_rows(cx, ninr, io.ninrflow, rows, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
     TV flow_t = A.tensor(Bk, H, W, 2);
     unnormalize_flow(cx, ninr, scaler, flow_t);
-    if (io.flowt) store(flow_t, io.flowt, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
+    if (io.flowt) nhwc_to_nchw_rows(cx, flow_t, io.flowt, rows, (int64_t)2 * H * W, (int64_t)H * W, 1.f, 0.f, 0);
 
     // ---- frame_synthesize (gimmvfi_r.py:222-322)
     TV s0 = syn.batch(0, Bk), s1 = syn.batch(B, Bk);
@@ -1550,7 +1560,7 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
       resize_bilinear(cx, fl4.slice(2, 2), a1, 0.25f, 0.25f, 4.f, 0, ACT_NONE);
       resize_bilinear(cx, mask4, am, 0.25f, 0.25f, 1.f, 0, ACT_SIGMOID);
       warp_blend(cx, s0, s1, a0, a1, am, wb);
-      store(wb, io.img_warp_4, (int64_t)3 * H * W, (int64_t)H * W, 0.5f, 1.0f, 1);
+      nhwc_to_nchw_rows(cx, wb, io.img_warp_4, rows, (int64_t)3 * H * W, (int64_t)H * W, 0.5f, 1.0f, 1);
       A.release(mk);
     }
     // _amt_corr_scale_lookup(downsample=2)  (gimmvfi_r.py:494-507)
@@ -1580,8 +1590,8 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
       if (last) tap("syn.corr_4_hi", corr_hi);
     }
     if (last) { tap("syn.ft_4", ft_4); tap("syn.fl4", fl4); tap("syn.mask4", mask4); }
-    if (io.flowt0_4) store(fl4.slice(0, 2), io.flowt0_4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
-    if (io.flowt1_4) store(fl4.slice(2, 2), io.flowt1_4, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
+    if (io.flowt0_4) nhwc_to_nchw_rows(cx, fl4.slice(0, 2), io.flowt0_4, rows, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
+    if (io.flowt1_4) nhwc_to_nchw_rows(cx, fl4.slice(2, 2), io.flowt1_4, rows, (int64_t)2 * H4 * W4, (int64_t)H4 * W4, 1.f, 0.f, 0);
 
     // NewMultiFlowDecoder (fi_components.py:307-340)
     TV F0 = A.tensor(Bk, H, W, 6, 8), F1 = A.tensor(Bk, H, W, 6, 8), Mk = A.tensor(Bk, H, W, 3, 4), Rs = A.tensor(Bk, H, W, 9, 12);
@@ -1636,16 +1646,15 @@ void Engine::run(Ctx& cx, const Problem& P0, const IO& io, const FlowInputs* fin
       resize_bilinear(cx, wide(Rs), wide(Rsf), rinv, rinv, 1.f, 0, ACT_NONE);
       if (last) { tap("syn.F0f", F0f); tap("syn.F1f", F1f); tap("syn.Mkf", Mkf); tap("syn.Rsf", Rsf); }
     }
-    if (io.flowt0_1) store(F0f, io.flowt0_1, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
-    if (io.flowt1_1) store(F1f, io.flowt1_1, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
+    if (io.flowt0_1) nhwc_to_nchw_rows(cx, F0f, io.flowt0_1, rows, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
+    if (io.flowt1_1) nhwc_to_nchw_rows(cx, F1f, io.flowt1_1, rows, (int64_t)6 * Hf * Wf, (int64_t)Hf * Wf, 1.f, 0.f, 0);
     // multi_flow_combine + amt_comb_block at FULL resolution (fi_components.py:57-94)
     {
       TV w9 = A.tensor(Bk, Hf, Wf, 9, 12), mean3 = A.tensor(Bk, Hf, Wf, 3, 4), c18 = A.tensor(Bk, Hf, Wf, 18, 20), c3 = A.tensor(Bk, Hf, Wf, 3, 4);
       multi_flow_blend(cx, synf.batch(0, Bk), synf.batch(B, Bk), F0f, F1f, Mkf, Rsf, w9, mean3);
       N.conv7x("amt_comb_block.0", w9, c18, ACT_PRELU, N.V("amt_comb_block.1.weight"));
       N.conv7x("amt_comb_block.2", c18, c3);
-      if (qs) combine_output_rows(cx, mean3, c3, io.imgt_pred, rows);
-      else combine_output(cx, mean3, c3, io.imgt_pred + (int64_t)ti * B * 3 * Hf * Wf);
+      combine_output_rows(cx, mean3, c3, io.imgt_pred, rows);
       if (last) { tap("syn.w9", w9); tap("syn.mean3", mean3); tap("syn.c3", c3); }
     }
   }
@@ -1848,10 +1857,9 @@ static IO fake_io() {
 
 size_t Engine::plan_from_flow(const Problem& p) {
   need(Entry::FromFlow);
-  const IO io = fake_io();
   FlowInputs fin; fin.flows = kFake;
   for (int j = 0; j < 2; ++j) fin.feat4[j] = fin.feat8[j] = fin.fnet[j] = kFake;
-  return dry_run([&](Ctx& cx) { run(cx, p, io, &fin); });
+  return dry_run([&](Ctx& cx) { run(cx, p, fake_io(), schedule_batch(p), &fin); });
 }
 
 void Engine::forward_from_flow(const Problem& p, const IO& io, const FlowInputs& fin, void* workspace, size_t workspace_bytes, gvStream_t stream) {
@@ -1859,13 +1867,12 @@ void Engine::forward_from_flow(const Problem& p, const IO& io, const FlowInputs&
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: img_xs, coords, t and imgt_pred are required");
   if (!fin.flows || !fin.feat4[0] || !fin.feat4[1] || !fin.feat8[0] || !fin.feat8[1] || !fin.fnet[0] || !fin.fnet[1])
     throw std::runtime_error("gimmvfi: forward_from_flow needs flows, feat4[2], feat8[2] and fnet[2]");
-  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, &fin); });
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, schedule_batch(p), &fin); });
 }
 
 size_t Engine::plan(const Problem& p) {
   need(Entry::Interpolate);
-  const IO io = fake_io();
-  return dry_run([&](Ctx& cx) { run(cx, p, io); });
+  return dry_run([&](Ctx& cx) { run(cx, p, fake_io(), schedule_batch(p)); });
 }
 
 void Engine::clear_graphs() {
@@ -1879,6 +1886,7 @@ void Engine::clear_graphs() {
 void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
   need(Entry::Interpolate);
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: img_xs, coords, t and imgt_pred are required");
+  const Schedule s = schedule_batch(p);
   launch(workspace, workspace_bytes, stream, [&](Ctx& cx) {
 #ifndef GV_HOSTSIM
     // (the legacy default stream - handles 0 / 1 / 2 - cannot be captured: such callers run eagerly)
@@ -1900,7 +1908,7 @@ void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t wor
         cudaGraph_t graph = nullptr;
         cuda_ok(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCapture");
         try {
-          run(cx, p, io);
+          run(cx, p, io, s);
         } catch (...) {
           cudaStreamEndCapture(stream, &graph);
           if (graph) cudaGraphDestroy(graph);
@@ -1922,29 +1930,25 @@ void Engine::forward(const Problem& p, const IO& io, void* workspace, size_t wor
       }
     }
 #endif
-    run(cx, p, io);
+    run(cx, p, io, s);
   });
 }
 
 size_t Engine::plan_clip(const Problem& p, const Clip& c) {
   need(Entry::Interpolate);
-  const IO io = fake_io();
-  return dry_run([&](Ctx& cx) { run(cx, p, io, nullptr, &c); });
+  return dry_run([&](Ctx& cx) { run(cx, p, fake_io(), schedule_clip(p, c)); });
 }
 
 // (eager: a clip's launch sequence depends on its pair list, which the CUDA-graph key of forward() does not hold)
 void Engine::forward_clip(const Problem& p, const Clip& c, const IO& io, void* workspace, size_t workspace_bytes, gvStream_t stream) {
   need(Entry::Interpolate);
   if (!io.img_xs || !io.coords || !io.t || !io.imgt_pred) throw std::runtime_error("gimmvfi: frames, coords, t and imgt_pred are required");
-  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, nullptr, &c); });
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, schedule_clip(p, c)); });
 }
 
 size_t Engine::plan_queries(const Problem& p, const Queries& q) {
   need(Entry::Interpolate);
-  const QuerySchedule s = schedule_queries(q);
-  IO io = fake_io();
-  io.coords = io.t = nullptr;
-  return dry_run([&](Ctx& cx) { run(cx, p, io, nullptr, nullptr, &s); });
+  return dry_run([&](Ctx& cx) { run(cx, p, fake_io(), schedule_queries(p, q)); });
 }
 
 // (eager, as forward_clip)
@@ -1952,8 +1956,7 @@ void Engine::forward_queries(const Problem& p, const Queries& q, const IO& io, v
   need(Entry::Interpolate);
   if (!io.img_xs || !io.imgt_pred) throw std::runtime_error("gimmvfi: frames and imgt_pred are required");
   if (io.coords || io.t) throw std::runtime_error("gimmvfi: a query list's coordinates and t are made by the engine; io.coords and io.t must be null");
-  const QuerySchedule s = schedule_queries(q);
-  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, nullptr, nullptr, &s); });
+  launch(workspace, workspace_bytes, stream, [&](Ctx& cx) { run(cx, p, io, schedule_queries(p, q)); });
 }
 
 // ---------------------------------------------------------------------------

@@ -55,7 +55,7 @@ struct Queries {
   std::vector<int> src, tgt;
   std::vector<float> t;
 };
-struct QuerySchedule;   // engine.cu: the slot schedule of a query list
+struct Schedule;   // engine.cu: the frames, pairs, timesteps and output rows of one interpolation (run())
 
 // Outputs of an EXTERNAL bidirectional flow estimator at the network resolution (GIMM-VFI-F: FlowFormer, gimmvfi_f.py:114-138) in the
 // reference's NCHW layouts; with these the engine runs everything downstream of cal_bidirection_flow (forward_from_flow)
@@ -252,7 +252,9 @@ class Engine {
   void prefix_flow_estimator(std::initializer_list<const char*> children);
   size_t dry_run(const std::function<void(Ctx&)>& run);
   void launch(void* workspace, size_t workspace_bytes, gvStream_t stream, const std::function<void(Ctx&)>& run);
-  void run(Ctx& cx, const Problem& p, const IO& io, const FlowInputs* fin = nullptr, const Clip* clip = nullptr, const QuerySchedule* qs = nullptr);
+  // fin: the flow estimate of an external estimator, with the schedule of forward()
+  void run(Ctx& cx, const Problem& p, const IO& io, const Schedule& sched, const FlowInputs* fin = nullptr);
+  void frame_cache(Ctx& cx, const Problem& p, const TV& fmap, const TV& ni, const TV& feat4, const TV& feat8);
   void finalize_decoders();
   void finalize_flowformer();
   void pack_patch_conv(const std::string& name);

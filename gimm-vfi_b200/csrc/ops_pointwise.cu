@@ -102,13 +102,15 @@ struct NhwcToNchwRowsK {
     s(i - n * per);
   }
 };
-static void check_rows(const TV& src, const std::vector<int>& rows) {
+static bool consecutive_rows(const TV& src, const std::vector<int>& rows) {   // checks the rows; true: consecutive (the plain store applies)
   if ((int)rows.size() != src.n) throw std::runtime_error("store_rows: one destination row per sample is required");
   for (int r : rows) if (r < 0) throw std::runtime_error("store_rows: negative destination row");
+  for (size_t n = 0; n < rows.size(); ++n) if (rows[n] != rows[0] + (int)n) return false;
+  return true;
 }
 void nhwc_to_nchw_rows(Ctx& cx, const TV& src, float* dst, const std::vector<int>& rows, int64_t dst_sn, int64_t dst_sc, float scale, float shift,
                        int clamp01) {
-  check_rows(src, rows);
+  if (consecutive_rows(src, rows)) return nhwc_to_nchw(cx, src, dst + (int64_t)rows[0] * dst_sn, dst_sn, dst_sc, scale, shift, clamp01);
   for (int n0 = 0; n0 < src.n; n0 += kGatherMax) {
     const int cnt = std::min(src.n - n0, kGatherMax);
     NhwcToNchwRowsK k{};
@@ -1534,7 +1536,7 @@ struct CombineOutRowsK {
   }
 };
 void combine_output_rows(Ctx& cx, const TV& mean3, const TV& conv3, float* dst_nchw, const std::vector<int>& rows) {
-  check_rows(mean3, rows);
+  if (consecutive_rows(mean3, rows)) return combine_output(cx, mean3, conv3, dst_nchw + (int64_t)rows[0] * 3 * mean3.h * mean3.w);
   for (int n0 = 0; n0 < mean3.n; n0 += kGatherMax) {
     const int cnt = std::min(mean3.n - n0, kGatherMax);
     CombineOutRowsK k{};
