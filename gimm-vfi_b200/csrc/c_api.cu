@@ -745,6 +745,16 @@ int gimmvfi_op_forward_interpolate(const float* flow, int n, int h, int w, float
     forward_interpolate(cx, flow, n, h, w, out);
   })
 }
+int gimmvfi_op_scene_sums(const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums, void* stream) {
+  gimmvfi_engine* e = nullptr;
+  GV_TRY(e, {
+    if (n < 0 || h < 1 || w < 1) throw std::runtime_error("scene_sums: n must be >= 0, h and w >= 1");
+    if ((int64_t)h * w >= ((int64_t)1 << 31)) throw std::runtime_error("scene_sums: h * w must be below 2^31");
+    if (n > 0 && (!a || !b || !sums)) throw std::runtime_error("scene_sums: a, b and sums are required");
+    Ctx cx = op_ctx(stream);
+    scene_sums(cx, a, b, n, h, w, sums);
+  })
+}
 int gimmvfi_op_pixel_shuffle(const gimmvfi_view* src, const gimmvfi_view* dst, int times, void* stream) {
   gimmvfi_engine* e = nullptr;
   GV_TRY(e, { Ctx cx = op_ctx(stream); pixel_shuffle(cx, to_tv(src), to_tv(dst), times); })

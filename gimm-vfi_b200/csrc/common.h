@@ -450,6 +450,9 @@ void pred_to_u8(Ctx& cx, const float* src_nchw, int n, int H, int W, uint8_t* ds
 struct FlowView { const float* p = nullptr; int64_t sn = 0, sy = 0, sx = 0, sc = 0; int n = 0, h = 0, w = 0; };
 int64_t flow_to_image_scratch_floats(int n, int h);
 void flow_to_image(Ctx& cx, const FlowView& flow, int has_clip, float clip, int has_max, float max_div, int bgr, float* scratch, uint8_t* dst);
+// scene-cut sums of n frame pairs: a, b (n,h,w,3) uint8 RGB, pair i = (a[i], b[i]) -> sums[i] = (sum |dH|, sum |dS|, sum |dV|) of
+// their 8-bit HSV (cv2.COLOR_RGB2HSV); every sum written, bit-exact on every run
+void scene_sums(Ctx& cx, const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums);
 // forward_interpolate (raft/utils/utils.py:33-63) of n dense (2,h,w) flows -> out (n,2,h,w), which must not overlap flow
 void forward_interpolate(Ctx& cx, const float* flow, int n, int h, int w, float* out);
 void pad_image4(Ctx& cx, const TV& src /*c=3, ld=4*/, const TV& dst /*h+2p, w+2p, ld 4*/, int pad);

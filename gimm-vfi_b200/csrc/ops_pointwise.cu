@@ -1734,4 +1734,153 @@ void lpips_head_images(Ctx& cx, const double* const partial[5], const int h[5], 
 #endif
 }
 
+// ---- scene-cut score: PySceneDetect's ContentDetector content value of consecutive uint8 RGB frames ----
+// cv2.cvtColor(x, COLOR_RGB2HSV) for 8-bit input in integers (H in [0, 180), S and V in [0, 255]; OpenCV's own fixed-point form):
+// sdiv[v] = round(255 * 4096 / v), hdiv[d] = round(180 * 4096 / (6 d)), both 0 at 0.  No quotient falls on a tie, so the integer
+// rounding (2a + b) / (2b) is exact.  The tables are built once on the host and ride in the kernel parameters.
+GV_HD int scene_sdiv(int v) { return v ? (2 * 255 * 4096 + v) / (2 * v) : 0; }
+GV_HD int scene_hdiv(int d) { return d ? (2 * 180 * 4096 + 6 * d) / (12 * d) : 0; }
+struct SceneTables { int sdiv[256], hdiv[256]; };
+static SceneTables scene_tables() {
+  SceneTables t;
+  for (int i = 0; i < 256; ++i) { t.sdiv[i] = scene_sdiv(i); t.hdiv[i] = scene_hdiv(i); }
+  return t;
+}
+// one pixel's HSV (v == r wins over v == g, as in OpenCV; the shift of a negative hue is arithmetic)
+GV_HD void scene_hsv(int r, int g, int b, const int* sdiv, const int* hdiv, int& H, int& S, int& V) {
+  const int v = r > g ? (r > b ? r : b) : (g > b ? g : b);
+  const int d = v - (r < g ? (r < b ? r : b) : (g < b ? g : b));
+  S = (d * sdiv[v] + 2048) >> 12;
+  const int h0 = v == r ? g - b : (v == g ? b - r + 2 * d : r - g + 4 * d);
+  const int h = (h0 * hdiv[d] + 2048) >> 12;
+  H = h < 0 ? h + 180 : h;
+  V = v;
+}
+// |dH|, |dS|, |dV| of one pixel of a (bytes pa) and b (bytes pb), added to acc
+GV_HD void scene_pixel(int ra, int ga, int ba, int rb, int gb, int bb, const int* sdiv, const int* hdiv, uint32_t acc[3]) {
+  int h0, s0, v0, h1, s1, v1;
+  scene_hsv(ra, ga, ba, sdiv, hdiv, h0, s0, v0);
+  scene_hsv(rb, gb, bb, sdiv, hdiv, h1, s1, v1);
+  acc[0] += (uint32_t)(h0 > h1 ? h0 - h1 : h1 - h0);
+  acc[1] += (uint32_t)(s0 > s1 ? s0 - s1 : s1 - s0);
+  acc[2] += (uint32_t)(v0 > v1 ? v0 - v1 : v1 - v0);
+}
+// the three sums of pixels p0, p0 + step, ... < P of pair (pa, pb); the caller keeps a thread's pixels below 2^32 / 255
+GV_HD void scene_pixels(const uint8_t* pa, const uint8_t* pb, int64_t p0, int64_t P, int64_t step, const int* sdiv, const int* hdiv, uint32_t acc[3]) {
+  for (int64_t p = p0; p < P; p += step) {
+    const uint8_t* x = pa + p * 3; const uint8_t* y = pb + p * 3;
+    scene_pixel(x[0], x[1], x[2], y[0], y[1], y[2], sdiv, hdiv, acc);
+  }
+}
+// host simulation: one pair per item, in runs of 2^16 pixels, every sum stored
+struct SceneSumsK {
+  const uint8_t* a; const uint8_t* b; int64_t P; uint64_t* sums; SceneTables t;
+  GV_HD void operator()(int64_t i) const {
+    uint64_t s[3] = {0, 0, 0};
+    for (int64_t p0 = 0; p0 < P; p0 += 65536) {
+      const int64_t cnt = P - p0 < 65536 ? P - p0 : 65536;
+      uint32_t acc[3] = {0, 0, 0};
+      scene_pixels(a + (i * P + p0) * 3, b + (i * P + p0) * 3, 0, cnt, 1, t.sdiv, t.hdiv, acc);
+      for (int c = 0; c < 3; ++c) s[c] += acc[c];
+    }
+    for (int c = 0; c < 3; ++c) sums[i * 3 + c] = s[c];
+  }
+};
+#ifndef GV_HOSTSIM
+constexpr int kSceneThreads = 256;
+constexpr int64_t kSceneSmallPixels = 64;   // frames up to this size: one thread per pair
+__device__ __forceinline__ void scene_load_tables(const SceneTables& t, int* sdiv, int* hdiv) {
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) { sdiv[i] = t.sdiv[i]; hdiv[i] = t.hdiv[i]; }
+  __syncthreads();
+}
+// small frames (the 2^24 1x1 pairs of an all-colours check): a thread owns a pair, so it stores its sums; the loads of a warp
+// cover 32 consecutive frames
+__global__ void __launch_bounds__(kSceneThreads) scene_sums_small_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, int n,
+                                                                       int64_t P, unsigned long long* __restrict__ sums, const __grid_constant__ SceneTables t) {
+  __shared__ int sdiv[256], hdiv[256];
+  scene_load_tables(t, sdiv, hdiv);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    uint32_t acc[3] = {0, 0, 0};
+    scene_pixels(a + i * P * 3, b + i * P * 3, 0, P, 1, sdiv, hdiv, acc);
+    for (int c = 0; c < 3; ++c) sums[i * 3 + c] = acc[c];
+  }
+}
+// byte j of 12 little-endian words
+__device__ __forceinline__ int scene_byte(const uint32_t* w, int j) { return (int)((w[j >> 2] >> ((j & 3) * 8)) & 0xffu); }
+// larger frames: CTA k of a pair's `per_pair` takes every per_pair-th block of 256 units (16 pixels = 3 x 16-byte loads per frame when
+// `vec`, else one pixel); the CTA's sums are reduced in registers and shared memory and added with one 64-bit atomic per channel
+__global__ void __launch_bounds__(kSceneThreads) scene_sums_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, int64_t P,
+                                                                 int per_pair, int vec, unsigned long long* __restrict__ sums,
+                                                                 const __grid_constant__ SceneTables t) {
+  __shared__ int sdiv[256], hdiv[256];
+  __shared__ unsigned long long red[kSceneThreads / 32][3];
+  scene_load_tables(t, sdiv, hdiv);
+  const int64_t pair = blockIdx.x / per_pair;
+  const int k = blockIdx.x % per_pair;
+  const uint8_t* pa = a + pair * P * 3;
+  const uint8_t* pb = b + pair * P * 3;
+  const int64_t first = (int64_t)k * kSceneThreads + threadIdx.x, step = (int64_t)per_pair * kSceneThreads;
+  uint32_t acc[3] = {0, 0, 0};
+  if (vec) {
+    const uint4* qa = reinterpret_cast<const uint4*>(pa);
+    const uint4* qb = reinterpret_cast<const uint4*>(pb);
+    for (int64_t g = first; g < P / 16; g += step) {
+      uint32_t wa[12], wb[12];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const uint4 x = __ldcs(qa + g * 3 + j), y = __ldcs(qb + g * 3 + j);
+        wa[4 * j] = x.x; wa[4 * j + 1] = x.y; wa[4 * j + 2] = x.z; wa[4 * j + 3] = x.w;
+        wb[4 * j] = y.x; wb[4 * j + 1] = y.y; wb[4 * j + 2] = y.z; wb[4 * j + 3] = y.w;
+      }
+#pragma unroll
+      for (int p = 0; p < 16; ++p)
+        scene_pixel(scene_byte(wa, 3 * p), scene_byte(wa, 3 * p + 1), scene_byte(wa, 3 * p + 2),
+                    scene_byte(wb, 3 * p), scene_byte(wb, 3 * p + 1), scene_byte(wb, 3 * p + 2), sdiv, hdiv, acc);
+    }
+  } else {
+    scene_pixels(pa, pb, first, P, step, sdiv, hdiv, acc);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    unsigned long long s = acc[c];
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) red[warp][c] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < 3) {
+    unsigned long long s = 0;
+    for (int w = 0; w < kSceneThreads / 32; ++w) s += red[w][threadIdx.x];
+    if (s) atomicAdd(sums + pair * 3 + threadIdx.x, s);
+  }
+}
+#endif
+void scene_sums(Ctx& cx, const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums) {
+  if (cx.dry || n <= 0) return;
+  const int64_t P = (int64_t)h * w;
+  const SceneTables t = scene_tables();
+#ifdef GV_HOSTSIM
+  parallel_for(cx, n, SceneSumsK{a, b, P, sums, t}, "scene_sums");
+#else
+  const int64_t cap = (int64_t)cx.sm_count * 8;
+  cx.launches++;
+  if (cx.prof) cx.prof->begin(cx.stream, "scene_sums", (double)n * P * 6.0);
+  unsigned long long* s = reinterpret_cast<unsigned long long*>(sums);
+  if (P <= kSceneSmallPixels) {
+    const int64_t blocks = std::min(((int64_t)n + kSceneThreads - 1) / kSceneThreads, cap);
+    scene_sums_small_kernel<<<(unsigned)blocks, kSceneThreads, 0, cx.stream>>>(a, b, n, P, s, t);
+  } else {
+    // 16-pixel units when every pair starts on a 16-byte boundary in both stacks (3 P % 16 == 0 <=> P % 16 == 0)
+    const int vec = aligned(a, 16) && aligned(b, 16) && P % 16 == 0;
+    const int64_t units = vec ? P / 16 : P;
+    const int64_t per_pair = std::max<int64_t>(1, std::min((units + kSceneThreads - 1) / kSceneThreads, cap / n));
+    const cudaError_t er = cudaMemsetAsync(sums, 0, (size_t)n * 3 * sizeof(uint64_t), cx.stream);
+    if (er != cudaSuccess) throw std::runtime_error(std::string("scene_sums: cudaMemsetAsync: ") + cudaGetErrorString(er));
+    scene_sums_kernel<<<(unsigned)(n * per_pair), kSceneThreads, 0, cx.stream>>>(a, b, P, (int)per_pair, vec, s, t);
+  }
+  gv_check_launch("scene_sums");
+  if (cx.prof) cx.prof->end(cx.stream);
+#endif
+}
+
 }  // namespace gv

@@ -470,6 +470,12 @@ int gimmvfi_op_flow_to_image(const float* flow, int64_t stride_n, int64_t stride
  * out NaN everywhere, as from the reference.  n*h*w*h*w float64 distances; no workspace; deterministic.
  * Refuses n, h or w < 1, n > 65535, h*w >= 2^31 and overlapping buffers. */
 int gimmvfi_op_forward_interpolate(const float* flow, int n, int h, int w, float* out, void* stream);
+/* Scene-cut sums of n frame pairs (the content value of PySceneDetect's ContentDetector): a, b (n,h,w,3) uint8 RGB, contiguous, on the
+ * device; pair i is (a[i], b[i]).  Both frames go to 8-bit HSV as cv2.cvtColor(x, COLOR_RGB2HSV) does (H in [0,180), S, V in [0,255]),
+ * and sums (n,3) uint64 on the device receives (sum |H_a - H_b|, sum |S_a - S_b|, sum |V_a - V_b|) over every pixel, H not wrapped.
+ * Every sum is written (the op zeroes what it accumulates into).  Integer sums: bit-exact on every run.  The score is
+ * (sums[i][0] + sums[i][1] + sums[i][2]) / (3 h w).  Refuses n < 0, h or w < 1 and h*w >= 2^31. */
+int gimmvfi_op_scene_sums(const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums, void* stream);
 /* nn.PixelShuffle(2) applied `times` times */
 int gimmvfi_op_pixel_shuffle(const gimmvfi_view* src, const gimmvfi_view* dst, int times, void* stream);
 

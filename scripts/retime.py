@@ -2,12 +2,14 @@
 interpolated by GIMM-VFI where that time falls between two input frames, the input frame itself where it falls on one.
 
     python scripts/retime.py --source-path frames/ --output-path out/ --fps-in 24 --fps-out 60 [--ds-factor 0.5] [--pairs-per-call 4]
-                             [--frames] [-m config.yaml] [-l ckpt.pth]
+                             [--scene-threshold 27] [--frames] [-m config.yaml] [-l ckpt.pth]
 
 Rates are exact rationals: 24, 30000/1001 or 29.97.  Frames are read in sorted order with cv2 (BGR converted to RGB); padding, the
 interpolation and the uint8 conversion run on the GPU (gimmvfi_b200.video.FrameRateConverter), K pairs per engine call.  Writes
 output.mp4 at fps_out, or numbered PNGs in output/ with --frames (and for frames larger than 2048 pixels when ffmpeg is missing, as
-video_nx.py).  Without -l the model has seeded weights."""
+video_nx.py).  --scene-threshold T: a pair of consecutive input frames whose scene-cut score (gimmvfi_b200.video.scene_scores) is
+>= T is a hard cut and is not interpolated; its output instants show the nearer input frame, and the cuts are listed at the end.
+Off unless given.  Without -l the model has seeded weights."""
 import argparse
 import os
 import sys
@@ -34,6 +36,8 @@ def parse_args(argv=None):
     p.add_argument("--pairs-per-call", type=int, default=1,
                    help="frame pairs interpolated per engine call, each frame encoded once (the workspace grows with it)")
     p.add_argument("--frames", action="store_true", help="write a PNG sequence output/%%04d.png instead of output.mp4")
+    p.add_argument("--scene-threshold", type=float, default=None,
+                   help="do not interpolate across a scene cut: a pair scoring >= this is one (27 is PySceneDetect's default); off if not given")
     return p.parse_args(argv)
 
 
@@ -48,7 +52,8 @@ def main(argv=None):
     os.makedirs(args.output_path, exist_ok=True)
     model = build_model(args, dev)
     ds = None if args.ds_factor == 1.0 else args.ds_factor   # a resize by 1 is the identity
-    conv = FrameRateConverter(model, args.fps_in, args.fps_out, ds_factor=ds, bgr=True, pairs_per_call=args.pairs_per_call)
+    conv = FrameRateConverter(model, args.fps_in, args.fps_out, ds_factor=ds, bgr=True, pairs_per_call=args.pairs_per_call,
+                              scene_threshold=args.scene_threshold)
     out = FrameSink(os.path.join(args.output_path, "output.mp4"), os.path.join(args.output_path, "output"), float(conv.fps_out), args.frames)
     for j, name in enumerate(names):
         bgr = cv2.imread(os.path.join(args.source_path, name), cv2.IMREAD_COLOR)
@@ -61,6 +66,8 @@ def main(argv=None):
         out.write(fr.cpu().numpy())
     out.close()
     print("wrote %d frames at %s fps to %s" % (out.count, conv.fps_out, args.output_path))
+    if args.scene_threshold is not None:
+        print("scene cuts (input frame j starts a new shot): %s" % (conv.cuts,))
 
 
 if __name__ == "__main__":

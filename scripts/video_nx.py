@@ -10,7 +10,9 @@ with_flow=True); only uint8 frames cross to the host.  The frame sequence is the
 pair the N-1 interpolated frames next to the pair's first frame, then the pair's second frame doubled, the very last one
 dropped (images[:-1]), at 2N fps.  --frames writes numbered PNGs into output/ and flow/ instead of videos; this is also what
 happens to a video whose frames the reference hands to ffmpeg (max(height, width // 2) > 2048) when ffmpeg is not installed.
-Without -l the model has seeded weights."""
+--scene-threshold T (off unless given): a pair whose scene-cut score (gimmvfi_b200.video.scene_scores) is >= T is a hard cut and is
+not interpolated; its N-1 frames are the nearer original and its flow pictures those of a zero flow, and the cuts are listed at the
+end.  Without -l the model has seeded weights."""
 import argparse
 import os
 import shutil
@@ -38,6 +40,8 @@ def parse_args(argv=None):
     p.add_argument("--frames", action="store_true", help="write PNG sequences output/%%04d.png and flow/%%04d.png instead of videos")
     p.add_argument("--pairs-per-call", type=int, default=1,
                    help="interpolate K consecutive pairs per engine call, each frame encoded once (1: one call per pair)")
+    p.add_argument("--scene-threshold", type=float, default=None,
+                   help="do not interpolate across a scene cut: a pair scoring >= this is one (27 is PySceneDetect's default); off if not given")
     return p.parse_args(argv)
 
 
@@ -101,7 +105,8 @@ def main(argv=None):
     out = FrameSink(os.path.join(args.output_path, "output.mp4"), os.path.join(args.output_path, "output"), fps, args.frames)
     flow = FrameSink(os.path.join(args.output_path, "flow.mp4"), os.path.join(args.output_path, "flow"), fps, args.frames)
     ds = None if args.ds_factor == 1.0 else args.ds_factor   # a resize by 1 is the identity
-    vi = VideoInterpolator(model, N=args.N, ds_factor=ds, bgr=True, with_flow=True, pairs_per_call=args.pairs_per_call)
+    vi = VideoInterpolator(model, N=args.N, ds_factor=ds, bgr=True, with_flow=True, pairs_per_call=args.pairs_per_call,
+                           scene_threshold=args.scene_threshold)
     host = lambda x: x.cpu().numpy()
     waiting = []   # originals whose interpolated frames have not come back yet (pairs_per_call > 1), oldest first
     per_pair = args.N - 1
@@ -133,6 +138,8 @@ def main(argv=None):
     out.close()
     flow.close()
     print("wrote %d frames and %d flow pictures to %s" % (out.count, flow.count, args.output_path))
+    if args.scene_threshold is not None:
+        print("scene cuts (input frame j starts a new shot): %s" % (vi.cuts,))
 
 
 if __name__ == "__main__":
