@@ -152,6 +152,25 @@ def flow_images(padder: InputPadder, flowt: List[torch.Tensor], bgr: bool) -> Li
     return out
 
 
+def _forward_pair(model, x0: torch.Tensor, x1: torch.Tensor, N: int, ds_factor: Optional[float], aux, frame_cache=None):
+    """model._interpolate on one pair of padded (3,H,W) frames at t = i/N, i = 1 .. N-1, the coordinates sample_coord_input's at
+    ds_factor.  frame_cache: None, or (buffer, load, store) as EngineHandle.forward takes it.  The engine keeps its own record of what a
+    buffer holds (problem size, precision mode; cleared when the weights change), and a load it refuses is retried once as a full
+    forward with load=False."""
+    dev = x0.device
+    xs = torch.stack([x0, x1], 1).unsqueeze(0).contiguous()          # (1,3,2,H,W)
+    H, W = xs.shape[-2:]
+    ratio = 1.0 if ds_factor is None else ds_factor
+    coords = [(model.sample_coord_input(1, (H, W), [i / N], device=dev, upsample_ratio=ratio), None) for i in range(1, N)]
+    ts = [i / N * torch.ones(1, device=dev) for i in range(1, N)]
+    try:
+        return model._interpolate(xs, coords, ts, ds_factor, aux, frame_cache=frame_cache)
+    except GimmvfiError as ex:
+        if not (frame_cache is not None and frame_cache[1] and "frame cache" in str(ex)):
+            raise
+        return model._interpolate(xs, coords, ts, ds_factor, aux, frame_cache=(frame_cache[0], False, frame_cache[2]))
+
+
 @torch.no_grad()
 def interpolate_pair_u8(model, frame0_u8: torch.Tensor, frame1_u8: torch.Tensor, N: int = 2, ds_factor: Optional[float] = None,
                         bgr: bool = True, with_flow: bool = False):
@@ -159,26 +178,122 @@ def interpolate_pair_u8(model, frame0_u8: torch.Tensor, frame1_u8: torch.Tensor,
     (h,w,3) uint8 frames at t = i/N.  with_flow: returns (frames, flow_images), the second being the N-1 colour-wheel pictures
     of the motion flowt (video_Nx.py:183-189, BGR when `bgr`), uint8 (h',w',3) on the device; only flowt is requested from the
     model besides the frames."""
-    dev = frame0_u8.device
     padder = InputPadder(frame0_u8.shape[:2], 32)
     x = padder.pad_u8(torch.stack([frame0_u8, frame1_u8], 0))          # (2,3,H,W)
-    xs = torch.stack([x[0], x[1]], 1).unsqueeze(0).contiguous()          # (1,3,2,H,W)
-    H, W = xs.shape[-2:]
-    ratio = 1.0 if ds_factor is None else ds_factor
-    coords = [(model.sample_coord_input(1, (H, W), [i / N], device=dev, upsample_ratio=ratio), None) for i in range(1, N)]
-    ts = [i / N * torch.ones(1, device=dev) for i in range(1, N)]
-    out = model._interpolate(xs, coords, ts, ds_factor, ("flowt",) if with_flow else False)
+    out = _forward_pair(model, x[0], x[1], N, ds_factor, ("flowt",) if with_flow else False)
     frames = [padder.unpad_u8(im, bgr)[0] for im in out["imgt_pred"]]
     return (frames, flow_images(padder, out["flowt"], bgr)) if with_flow else frames
 
 
-class VideoInterpolator:
+class _Stream:
+    """What VideoInterpolator and FrameRateConverter share: a clip's input frames, pushed one by one, become a stream of outputs.  Pushing
+    input frame j schedules the output instants in (j - 1, j] (the subclass's _instants).  An output is an input frame passed through, or
+    the interpolation of the pair (j - 1, j) at some t, which falls back to the nearer input frame (offset <= 1/2: the earlier) if the
+    pair turns out to be a scene cut.  The outputs wait in a queue in output order.  A push that leaves no interpolation waiting returns
+    the queue and reads nothing back.  A push that brings the distinct pairs waiting to pairs_per_call, and flush(), read every waiting
+    scene score in one copy, turn the entries of cut pairs into their fallback frames, and send the pairs left to one engine call (the
+    subclass's _run) on only the frames they use; then the whole queue comes back in order."""
+
+    with_flow = False
+    _passes_frames = False   # whether an output instant can fall on an input frame (then uint8 copies are always kept)
+
+    def __init__(self, model, ds_factor: Optional[float], bgr: bool, pairs_per_call: int, scene_threshold: Optional[float]):
+        self.scene_threshold = _scene_threshold(scene_threshold)
+        self.model, self.ds, self.bgr, self.pairs_per_call = model, ds_factor, bgr, int(pairs_per_call)
+        self._padder = None
+        self._scene = None if self.scene_threshold is None else _Cuts(self.scene_threshold)
+        # uint8 copies of the input frames, kept only where an output can be one: a pass-through frame or a cut's fallback
+        self._copies = self._passes_frames or self._scene is not None
+        self.reset()
+
+    @property
+    def cuts(self) -> List[int]:
+        return list(self._scene.cuts) if self._scene is not None else []
+
+    def reset(self):
+        """start a new clip: the next frame pushed is input frame 0"""
+        self._n = 0             # input frames pushed
+        # the scheduled outputs, in order: ((j - 1, j), t, fallback) for an interpolation, (None, None, frame) for an input frame, the
+        # frames being our uint8 copies (None without copies)
+        self._queue = []
+        self._padded = {}       # input index -> padded float frame (3,H,W): the frames of the pairs waiting, and the last frame
+        self._last_u8 = None    # the copy of the last frame pushed
+        if self._scene is not None:
+            self._scene.reset()
+
+    def _net_size(self, H: int, W: int):
+        """the network-resolution size of padded H x W frames: sample_coord_input's grid at ds_factor"""
+        ratio = 1.0 if self.ds is None else self.ds
+        return int(H * ratio), int(W * ratio)
+
+    @torch.no_grad()
+    def flush(self):
+        """interpolate what is waiting and return every output scheduled, in order, as push() does; nothing is left waiting"""
+        return self._emit(True)
+
+    @torch.no_grad()
+    def push(self, frame_u8: torch.Tensor):
+        """the next input frame, (h,w,3) uint8 RGB on the device -> the outputs completed by it, in order (uint8 (h,w,3), BGR when `bgr`)"""
+        if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
+            if self._queue:
+                raise ValueError("%s: the frame size changed with outputs still waiting; flush() first" % type(self).__name__)
+            self._padder = InputPadder(frame_u8.shape[:2], 32)
+            self.reset()
+        j = self._n
+        self._n += 1
+        prev_u8, cur_u8 = self._last_u8, (frame_u8.clone() if self._copies else None)   # the caller may reuse its buffer
+        if self._scene is not None and j > 0:
+            self._scene.push(j, prev_u8, cur_u8)
+        if cur_u8 is None:   # the padded frame is then the only copy of frame j that the next pair can use
+            self._padded[j] = self._padder.pad_u8(frame_u8.unsqueeze(0))[0]
+        for off, t in self._instants(j):
+            fallback = prev_u8 if off <= Fraction(1, 2) else cur_u8
+            if t is None:
+                self._queue.append((None, None, fallback))
+                continue
+            for f, u8 in ((j - 1, prev_u8), (j, frame_u8)):
+                if f not in self._padded:
+                    self._padded[f] = self._padder.pad_u8(u8.unsqueeze(0))[0]
+            self._queue.append(((j - 1, j), t, fallback))
+        self._last_u8 = cur_u8
+        waiting = {pair for pair, _, _ in self._queue if pair is not None}
+        if waiting and len(waiting) < self.pairs_per_call:
+            return ([], []) if self.with_flow else []
+        return self._emit(bool(waiting))
+
+    def _emit(self, decide: bool):
+        """every output in the queue, in order, leaving it empty.  decide: read the waiting scene scores first and turn the entries of
+        cut pairs into their fallback frames.  An engine call that raises drops the outputs it was to make, and the clip goes on with the
+        next frame pushed."""
+        if decide and self._scene is not None:
+            self._scene.resolve()
+            self._queue = [(None, None, u8) if pair is not None and pair[1] in self._scene else (pair, t, u8) for pair, t, u8 in self._queue]
+        queue, self._queue = self._queue, []
+        interp = [(pair, t) for pair, t, _ in queue if pair is not None]
+        preds = flows = iter(())
+        if interp:
+            used = sorted({f for pair, _ in interp for f in pair})   # without a cut: every frame since the last call
+            local = {f: i for i, f in enumerate(used)}
+            ims, fl = self._run(used, [self._padded[f] for f in used], [(local[a], local[b], t) for (a, b), t in interp])
+            preds, flows = iter(self._padder.unpad_u8(ims, self.bgr).unbind(0)), iter(fl or ())
+        self._padded = {f: x for f, x in self._padded.items() if f == self._n - 1}
+        frames = [next(preds) if pair is not None else _as_output(u8, self.bgr) for pair, _, u8 in queue]
+        if not self.with_flow:
+            return frames
+        zero = None
+        if len(interp) < len(queue):   # a cut's pictures are those of a zero flow at the network resolution
+            zero = torch.zeros(2, *self._net_size(*self._padder.padded_shape), dtype=torch.float32, device=queue[0][2].device)
+        pics = [next(flows) if pair is not None else zero for pair, _, _ in queue]
+        return frames, (flow_images(self._padder, pics, self.bgr) if pics else [])
+
+
+class VideoInterpolator(_Stream):
     """video_Nx.py's frame loop (src/video_Nx.py:134-216) as a streaming object: push() the frames of a clip one by one and
-    get the N-1 interpolated frames between the previous frame and the new one.  Consecutive pairs share a frame, so the
-    RAFT encoder products of each pair's second frame (fnet map, cnet net/inp, projected context features) stay in a device
-    cache and are not recomputed when that frame becomes the next pair's first frame (SURVEY.md 8(f) row 2); the outputs
-    are bit-identical to independent per-pair calls.  with_flow: push() returns (frames, flow_images) as
-    interpolate_pair_u8(..., with_flow=True) does.
+    get the N-1 interpolated frames at t = i/N between the previous frame and the new one (N >= 2).  Consecutive pairs share a frame, so
+    the RAFT encoder products of each pair's second frame (fnet map, cnet net/inp, projected context features) stay in a device cache
+    and are not recomputed when that frame becomes the next pair's first frame (SURVEY.md 8(f) row 2); the outputs are bit-identical
+    to independent per-pair calls.  A pair loads the cache only when it holds the pair's first frame, under the same engine, precision
+    mode and weights.  with_flow: push() returns (frames, flow_images) as interpolate_pair_u8(..., with_flow=True) does.
 
     pairs_per_call K > 1: push() buffers frames until K pairs are waiting, then interpolates them in one model.interpolate call
     (K + 1 frames, each encoded once; the last is kept as the next call's first frame) and returns the K (N-1) frames in clip order,
@@ -190,151 +305,55 @@ class VideoInterpolator:
     `bgr`), and with_flow gives the colour-wheel picture of a zero flow for each.  The score of a pair is computed on the device when its
     second frame is pushed and read back once per engine call (K = 1: once per push; K > 1: once per block of K pairs, of which only the
     pairs that are not cuts go to the engine, and none at all when every pair is one).  `cuts` lists the input indices j whose pair
-    (j - 1, j) was a cut since the last reset().  With K = 1 the pair after a cut runs without the frame cache, which holds nothing of
-    its first frame."""
+    (j - 1, j) was a cut since the last reset().  With K = 1 the pair after a cut does not load the frame cache, which holds the products
+    of the frame before the cut."""
 
     def __init__(self, model, N: int = 2, ds_factor: Optional[float] = None, bgr: bool = True, with_flow: bool = False,
                  pairs_per_call: int = 1, scene_threshold: Optional[float] = None):
         if int(pairs_per_call) < 1:
             raise ValueError("pairs_per_call must be >= 1, got %r" % (pairs_per_call,))
-        self.scene_threshold = _scene_threshold(scene_threshold)
-        self.model, self.N, self.ds, self.bgr, self.with_flow = model, int(N), ds_factor, bgr, bool(with_flow)
-        self.pairs_per_call = int(pairs_per_call)
-        self._prev = None      # padded float frame (3,H,W) of the last push
-        self._padder = None
-        self._cache = None     # uint8 device buffer holding the previous frame's encoder products
-        self._cache_valid = False
-        self._pending = []     # pairs_per_call > 1: the padded frames pushed after _prev, not yet interpolated
-        self._scene = None if self.scene_threshold is None else _Cuts(self.scene_threshold)
-        self._n = 0            # frames pushed since the last reset
-        self._u8 = []          # scene detection: copies of the uint8 frames of _prev and _pending
-
-    @property
-    def cuts(self) -> List[int]:
-        return list(self._scene.cuts) if self._scene is not None else []
+        if int(N) < 2:
+            raise ValueError("N must be >= 2 (the N - 1 frames between two input frames are at t = i / N), got %r" % (N,))
+        self.N, self.with_flow = int(N), bool(with_flow)
+        self._cache = None     # uint8 device buffer holding the encoder products of the frame self._cached names
+        super().__init__(model, ds_factor, bgr, pairs_per_call, scene_threshold)
 
     def reset(self):
-        self._prev, self._cache_valid, self._pending = None, False, []
-        self._n, self._u8 = 0, []
-        if self._scene is not None:
-            self._scene.reset()
+        super().reset()
+        self._cached = None    # (input index of the frame whose products the frame cache holds, signature), or None
 
-    def _empty(self):
-        return ([], []) if self.with_flow else []
+    def _instants(self, j: int):
+        return [(Fraction(i, self.N), i / self.N) for i in range(1, self.N)] if j > 0 else []
 
-    def _cut_frames(self, a_u8: torch.Tensor, b_u8: torch.Tensor):
-        """the N - 1 outputs of a cut pair: the nearer input frame at each t = i / N (ties to the earlier), and zero-flow pictures"""
-        N = self.N
-        frames = [_as_output(a_u8 if 2 * i <= N else b_u8, self.bgr) for i in range(1, N)]
-        if not self.with_flow:
-            return frames, []
-        H, W = self._padder.padded_shape
-        ratio = 1.0 if self.ds is None else self.ds
-        zero = torch.zeros(2, int(H * ratio), int(W * ratio), dtype=torch.float32, device=a_u8.device)
-        return frames, flow_images(self._padder, [zero] * (N - 1), self.bgr)
-
-    @torch.no_grad()
-    def flush(self):
-        """interpolate the pairs still buffered (pairs_per_call > 1) and return their frames as push() does; nothing is left waiting"""
-        if not self._pending:
-            return self._empty()
-        k = len(self._pending)
-        cut = [False] * k
-        if self._scene is not None:
-            self._scene.resolve()
-            cut = [self._n - k + p in self._scene for p in range(k)]   # pair p is (input n - k + p - 1, n - k + p)
-        keep = [p for p in range(k) if not cut[p]]
+    def _run(self, used, frames, queries):
+        """one engine call on the waiting pairs -> their predictions (n,3,H,W) and with_flow their flowt, in queue order"""
         N, aux = self.N, ("flowt",) if self.with_flow else False
-        frames_u8, flows = [], []
-        if keep:
-            # only the frames of the pairs that are sent: with no cut, every frame and the pairs (i, i + 1)
-            clip = [self._prev] + self._pending
-            used = sorted({f for p in keep for f in (p, p + 1)})
-            local = {f: i for i, f in enumerate(used)}
-            frames = torch.stack([clip[f] for f in used], 0)               # (k+1,3,H,W) without a cut
-            kk = len(keep)
-            out = self.model._interpolate_clip(frames, [(local[p], local[p + 1]) for p in keep], [i / N for i in range(1, N)], self.ds, aux)
-            # out["imgt_pred"][i] is (kk,3,H,W): timestep i of every pair -> clip order, pair by pair
-            ims = torch.stack(out["imgt_pred"], 1).reshape(kk * (N - 1), *out["imgt_pred"][0].shape[1:])
-            frames_u8 = list(self._padder.unpad_u8(ims, self.bgr).unbind(0)) if N > 1 else []
-            if self.with_flow:
-                fl = out["flowt"]   # T x (kk,2,Hc,Wc), or (2,Hc,Wc) when kk == 1 (forward's .squeeze())
-                fl = [f.reshape(kk, *f.shape[-3:]) for f in fl]
-                flows = flow_images(self._padder, [fl[i][p] for p in range(kk) for i in range(N - 1)], self.bgr)
-        self._prev, self._pending = self._pending[-1], []
-        if len(keep) < k:   # the cut pairs' frames in their places
-            got_f, got_fl, frames_u8, flows = iter(frames_u8), iter(flows), [], []
-            for p in range(k):
-                if cut[p]:
-                    f, fl = self._cut_frames(self._u8[p], self._u8[p + 1])
-                else:
-                    f = [next(got_f) for _ in range(N - 1)]
-                    fl = [next(got_fl) for _ in range(N - 1)] if self.with_flow else []
-                frames_u8 += f
-                flows += fl
-        if self._scene is not None:
-            self._u8 = self._u8[-1:]
-        return (frames_u8, flows) if self.with_flow else frames_u8
-
-    @torch.no_grad()
-    def push(self, frame_u8: torch.Tensor):
-        dev = frame_u8.device
-        if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
-            if self._pending:
-                raise ValueError("VideoInterpolator: the frame size changed with pairs still buffered; flush() first")
-            self._padder = InputPadder(frame_u8.shape[:2], 32)
-            self.reset()
-        cur = self._padder.pad_u8(frame_u8.unsqueeze(0))[0]              # (3,H,W)
-        j = self._n
-        self._n += 1
-        if self._scene is not None:
-            u8 = frame_u8.clone()   # the caller may reuse its buffer; a cut pair's outputs are these bytes
-            if self._u8:
-                self._scene.push(j, self._u8[-1], u8)
-            self._u8.append(u8)
-        if self._prev is None:
-            self._prev = cur
-            return self._empty()
+        pairs = list(dict.fromkeys((a, b) for a, b, _ in queries))
         if self.pairs_per_call > 1:
-            self._pending.append(cur)
-            return self.flush() if len(self._pending) == self.pairs_per_call else self._empty()
-        if self._scene is not None:
-            self._scene.resolve()
-            prev_u8, self._u8 = self._u8[0], self._u8[-1:]
-            if j in self._scene:
-                self._prev, self._cache_valid = cur, False   # the cache holds frame j - 1's products, not frame j's
-                frames, flows = self._cut_frames(prev_u8, self._u8[0])
-                return (frames, flows) if self.with_flow else frames
-        m = self.model
-        xs = torch.stack([self._prev, cur], 1).unsqueeze(0).contiguous()  # (1,3,2,H,W)
-        H, W = xs.shape[-2:]
-        ratio = 1.0 if self.ds is None else self.ds
-        N = self.N
-        coords = [(m.sample_coord_input(1, (H, W), [i / N], device=dev, upsample_ratio=ratio), None) for i in range(1, N)]
-        ts = [i / N * torch.ones(1, device=dev) for i in range(1, N)]
-        Hc, Wc = coords[0][0].shape[2:4]
-        need = m.engine.frame_cache_bytes(1, H, W, N - 1, self.ds, Hc, Wc)
+            out = self.model._interpolate_clip(torch.stack(frames, 0), pairs, [i / N for i in range(1, N)], self.ds, aux)
+        else:
+            out = self._forward_cached(used, frames, aux)
+        # out[key][i] holds timestep i of every pair -> queue order, pair by pair
+        P = len(pairs)
+        ims = torch.stack(out["imgt_pred"], 1).reshape(P * (N - 1), *out["imgt_pred"][0].shape[1:])
+        if not self.with_flow:
+            return ims, None
+        fl = [f.reshape(P, *f.shape[-3:]) for f in out["flowt"]]   # (2,Hc,Wc) for a single pair (forward's .squeeze())
+        return ims, [fl[i][p] for p in range(P) for i in range(N - 1)]
+
+    def _forward_cached(self, used, frames, aux):
+        """pairs_per_call 1: the pair's forward through the frame cache, loading it when it holds the pair's first frame"""
+        m, (a, b), dev = self.model, used, frames[0].device
+        H, W = frames[0].shape[-2:]
+        need = m.engine.frame_cache_bytes(1, H, W, self.N - 1, self.ds, *self._net_size(H, W))
         if self._cache is None or self._cache.numel() < need or self._cache.device != dev:
-            self._cache, self._cache_valid = torch.empty(need, dtype=torch.uint8, device=dev), False
-        aux = ("flowt",) if self.with_flow else False
-        # The engine keeps its own record of what each cache buffer holds (problem size, precision mode; cleared when the weights
-        # change): a refused load -> one full forward with load=False.  The signature adds what only the caller can know.
+            self._cache, self._cached = torch.empty(need, dtype=torch.uint8, device=dev), None
+        # the engine refuses a load its own record of the buffer does not match; the signature adds what only the caller can know
         sig = (id(m.engine), int(m.tensor_cores), m.engine.weights_version)
-        load = self._cache_valid and getattr(self, "_cache_sig", None) == sig
-        try:
-            try:
-                out = m._interpolate(xs, coords, ts, self.ds, aux, frame_cache=(self._cache, load, True))
-            except GimmvfiError as ex:
-                if not (load and "frame cache" in str(ex)):
-                    raise
-                out = m._interpolate(xs, coords, ts, self.ds, aux, frame_cache=(self._cache, False, True))
-            self._cache_valid, self._cache_sig = True, sig
-        except Exception:
-            self._cache_valid = False
-            raise
-        self._prev = cur
-        frames = [self._padder.unpad_u8(im, self.bgr)[0] for im in out["imgt_pred"]]
-        return (frames, flow_images(self._padder, out["flowt"], self.bgr)) if self.with_flow else frames
+        held, self._cached = self._cached, None   # after an exception, the cache holds nothing known
+        out = _forward_pair(m, frames[0], frames[1], self.N, self.ds, aux, frame_cache=(self._cache, held == (a, sig), True))
+        self._cached = (b, sig)
+        return out
 
 
 def _rate(x, name: str) -> Fraction:
@@ -353,7 +372,7 @@ def _rate(x, name: str) -> Fraction:
 SNAP = Fraction(1, 10 ** 6)   # output instants this close to an input frame (in input frames) are that frame
 
 
-class FrameRateConverter:
+class FrameRateConverter(_Stream):
     """Frame-rate conversion of a clip streamed frame by frame: push() the (h,w,3) uint8 RGB input frames, get the output frames at
     fps_out.  Output frame k shows input time tau_k = k * fps_in / fps_out (in input frames, exact rationals: no drift), for every k with
     tau_k <= the last input frame.  A tau_k within SNAP (1e-6 input frames) of an input frame is that frame itself (no engine work; its
@@ -374,81 +393,26 @@ class FrameRateConverter:
     engine call or flush(), when the K pairs with queries of a call are decided, and a call whose pairs are all cuts is not made.
     `cuts` lists the input indices j whose pair (j - 1, j) scored >= T since the last reset()."""
 
+    _passes_frames = True
+
     def __init__(self, model, fps_in, fps_out, ds_factor: Optional[float] = None, bgr: bool = True, pairs_per_call: int = 1,
                  scene_threshold: Optional[float] = None):
         if isinstance(pairs_per_call, bool) or int(pairs_per_call) < 1:
             raise ValueError("pairs_per_call must be >= 1, got %r" % (pairs_per_call,))
-        self.scene_threshold = _scene_threshold(scene_threshold)
-        self.model, self.ds, self.bgr, self.pairs_per_call = model, ds_factor, bgr, int(pairs_per_call)
+        super().__init__(model, ds_factor, bgr, pairs_per_call, scene_threshold)
         self.fps_in, self.fps_out = _rate(fps_in, "fps_in"), _rate(fps_out, "fps_out")
         self.step = self.fps_in / self.fps_out   # input frames per output frame
-        self._padder = None
-        self._scene = None if self.scene_threshold is None else _Cuts(self.scene_threshold)
-        self.reset()
-
-    @property
-    def cuts(self) -> List[int]:
-        return list(self._scene.cuts) if self._scene is not None else []
 
     def reset(self):
-        """start a new clip: the next frame pushed is input frame 0"""
-        self._n = 0             # input frames pushed
+        super().reset()
         self._k = 0             # next output index to schedule
-        self._prev_u8 = None    # a copy of the last frame pushed
-        # scheduled outputs, in order: ("frame", uint8 (h,w,3)) or ("query", src, tgt, t, the input frame shown if (src, tgt) is a cut)
-        self._queue = []
-        self._frames = {}       # input index -> padded float frame (3,H,W), for the queries waiting
-        if self._scene is not None:
-            self._scene.reset()
 
-    @torch.no_grad()
-    def flush(self) -> List[torch.Tensor]:
-        """interpolate the queries waiting and return every scheduled output frame, in order"""
-        return self._emit(True)
-
-    def _emit(self, decide: bool) -> List[torch.Tensor]:
-        """flush(); decide: read the waiting scene scores first (push() skips it when no query waits)"""
-        if decide and self._scene is not None:
-            self._scene.resolve()
-            self._queue = [("frame", _as_output(e[4], self.bgr)) if e[0] == "query" and e[2] in self._scene else e for e in self._queue]
-        queries = [e[1:4] for e in self._queue if e[0] == "query"]
-        preds = iter(())
-        if queries:
-            used = sorted({f for a, b, _ in queries for f in (a, b)})   # without a cut: every frame in self._frames
-            local = {f: i for i, f in enumerate(used)}
-            frames = torch.stack([self._frames[f] for f in used], 0)
-            out = self.model._interpolate_at(frames, [(local[a], local[b], t) for a, b, t in queries], self.ds, False)
-            preds = iter(self._padder.unpad_u8(out["imgt_pred"], self.bgr).unbind(0))
-        res = [e[1] if e[0] == "frame" else next(preds) for e in self._queue]
-        self._queue, self._frames = [], {}
-        return res
-
-    @torch.no_grad()
-    def push(self, frame_u8: torch.Tensor) -> List[torch.Tensor]:
-        """the next input frame, (h,w,3) uint8 RGB -> the output frames completed by it, in order (uint8 (h,w,3), BGR when `bgr`)"""
-        if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
-            if self._queue:
-                raise ValueError("FrameRateConverter: the frame size changed with frames still waiting; flush() first")
-            self._padder = InputPadder(frame_u8.shape[:2], 32)
-            self.reset()
-        j = self._n
-        self._n += 1
-        cur_u8 = frame_u8.clone()
-        if self._scene is not None and j > 0:
-            self._scene.push(j, self._prev_u8, cur_u8)
+    def _instants(self, j: int):
         while self._k * self.step <= j:   # the output instants in (j - 1, j] (frame 0: the instant 0)
             off = self._k * self.step - (j - 1)   # in (0, 1]
             self._k += 1
-            if off >= 1 - SNAP or off <= SNAP:    # input frame j, or (a hair after it) frame j - 1
-                self._queue.append(("frame", _as_output(cur_u8 if off >= 1 - SNAP else self._prev_u8, self.bgr)))
-                continue
-            for f, u8 in ((j - 1, self._prev_u8), (j, cur_u8)):
-                if f not in self._frames:
-                    self._frames[f] = self._padder.pad_u8(u8.unsqueeze(0))[0]
-            near = self._prev_u8 if off <= Fraction(1, 2) else cur_u8   # the output if (j - 1, j) is a cut
-            self._queue.append(("query", j - 1, j, float(np.float32(float(off))), near))
-        self._prev_u8 = cur_u8
-        waiting = {(e[1], e[2]) for e in self._queue if e[0] == "query"}
-        if not waiting:
-            return self._emit(False)
-        return self._emit(True) if len(waiting) >= self.pairs_per_call else []
+            # input frame j, or (a hair after it) frame j - 1; any other instant is interpolated at the float32 t the engine receives
+            yield off, None if off >= 1 - SNAP or off <= SNAP else float(np.float32(float(off)))
+
+    def _run(self, used, frames, queries):
+        return self.model._interpolate_at(torch.stack(frames, 0), queries, self.ds, False)["imgt_pred"], None

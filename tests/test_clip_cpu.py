@@ -164,6 +164,15 @@ def test_video_interpolator_refuses_bad_pairs_per_call():
         VideoInterpolator(_StubModel(), N=2, pairs_per_call=0)
 
 
+@pytest.mark.parametrize("N", [1, 0])
+def test_video_interpolator_refuses_n_below_2(N):
+    """N = 1 would schedule no frame between two inputs"""
+    from gimmvfi_b200.video import VideoInterpolator
+
+    with pytest.raises(ValueError, match="N must be >= 2"):
+        VideoInterpolator(_StubModel(), N=N)
+
+
 def test_video_interpolator_frame_size_change_needs_flush(stub_video):
     vi = stub_video.VideoInterpolator(_StubModel(), N=2, pairs_per_call=3)
     vi.push(_frame(0))

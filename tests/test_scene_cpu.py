@@ -1,6 +1,7 @@
 """Scene-cut detection without a GPU: the host-simulation build of gimmvfi_op_scene_sums against cv2's RGB -> HSV (every 8-bit colour, and
 random frames up to 1080x1920), the C export, and FrameRateConverter / VideoInterpolator with chosen scores and stub models: no engine work
-for a cut, the nearer input frame in its place, K grouping, `cuts`, the frame cache after a cut, and scene_threshold=None unchanged."""
+for a cut, the nearer input frame in its place, K grouping, `cuts`, when the K = 1 frame cache is loaded, and scene_threshold=None
+unchanged."""
 import ctypes as C
 import math
 import os
@@ -384,6 +385,66 @@ def test_interpolator_threshold_without_cuts_matches_none(V, monkeypatch, K):
     m, vi, out, fl = _run_vi(V, 4, K, 8, threshold=27, with_flow=True)
     assert m.calls == ref_m.calls
     assert all(torch.equal(a, b) for a, b in zip(out + fl, ref + ref_fl)) and len(out + fl) == len(ref + ref_fl)
+
+
+class _FailingModel(_StubModel):
+    """_StubModel whose calls with the given numbers (counted from 0) raise the given exception after they are recorded"""
+
+    def __init__(self, fail):
+        super().__init__()
+        self.fail = fail
+
+    def _interpolate(self, xs, coords, ts, ds, aux, frame_cache=None):
+        out = super()._interpolate(xs, coords, ts, ds, aux, frame_cache)
+        if len(self.calls) - 1 in self.fail:
+            raise self.fail[len(self.calls) - 1]
+        return out
+
+
+def _push_all(vi, frames):
+    for j in frames:
+        vi.push(_frame(j))
+
+
+def test_interpolator_retries_a_refused_cache_load_once(V):
+    """the engine refuses the load of pair (1,2): one full forward of that pair, and the next pair loads again"""
+    from gimmvfi_b200._lib import GimmvfiError
+
+    m = _FailingModel({1: GimmvfiError("frame cache: the buffer holds another problem size")})
+    vi = V.VideoInterpolator(m, N=2)
+    _push_all(vi, range(4))
+    assert [c[1:] for c in m.calls] == [((0, 1), False), ((1, 2), True), ((1, 2), False), ((2, 3), True)]
+    # a refusal of the full forward too is not retried again
+    m = _FailingModel({1: GimmvfiError("frame cache: refused"), 2: GimmvfiError("frame cache: refused")})
+    vi = V.VideoInterpolator(m, N=2)
+    _push_all(vi, range(2))
+    with pytest.raises(GimmvfiError):
+        vi.push(_frame(2))
+    assert [c[1:] for c in m.calls] == [((0, 1), False), ((1, 2), True), ((1, 2), False)]
+
+
+@pytest.mark.parametrize("change", ["tensor_cores", "weights_version"])
+def test_interpolator_cache_not_loaded_after_a_precision_or_weights_change(V, change):
+    m = _StubModel()
+    vi = V.VideoInterpolator(m, N=2)
+    _push_all(vi, range(3))
+    if change == "tensor_cores":
+        m.tensor_cores = 1
+    else:
+        m.engine.weights_version = 1
+    _push_all(vi, range(3, 5))
+    assert [c[1:] for c in m.calls] == [((0, 1), False), ((1, 2), True), ((2, 3), False), ((3, 4), True)]
+
+
+def test_interpolator_cache_not_loaded_after_an_engine_error(V):
+    """pair (2,3) fails: the next pair does not load, and the clip goes on from frame 3"""
+    m = _FailingModel({2: RuntimeError("engine failure")})
+    vi = V.VideoInterpolator(m, N=2)
+    _push_all(vi, range(3))
+    with pytest.raises(RuntimeError, match="engine failure"):
+        vi.push(_frame(3))
+    _push_all(vi, range(4, 6))
+    assert [c[1:] for c in m.calls] == [((0, 1), False), ((1, 2), True), ((2, 3), True), ((3, 4), False), ((4, 5), True)]
 
 
 def test_interpolator_frame_size_change_starts_a_new_clip(V, monkeypatch):
