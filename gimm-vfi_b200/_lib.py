@@ -82,7 +82,7 @@ EXPORTS = [
     "gimmvfi_op_softsplat_out", "gimmvfi_op_softsplat_grad",
     "gimmvfi_op_alt_corr_forward", "gimmvfi_op_alt_corr_backward",
     "gimmvfi_op_forward_interpolate",
-    "gimmvfi_op_scene_sums",
+    "gimmvfi_op_scene_sums", "gimmvfi_op_blend_u8",
     "gimmvfi_set_motion_config",
     "gimmvfi_plan_clip", "gimmvfi_forward_clip",
     "gimmvfi_plan_queries", "gimmvfi_forward_queries", "gimmvfi_set_coord_range",
@@ -199,6 +199,7 @@ class Lib:
         d.gimmvfi_op_alt_corr_backward.argtypes = [PD, PD, PD, PD, i32, PD, PD, PD, vp]
         d.gimmvfi_op_forward_interpolate.argtypes = [vp, i32, i32, i32, vp, vp]
         d.gimmvfi_op_scene_sums.argtypes = [vp, vp, i32, i32, i32, vp, vp]
+        d.gimmvfi_op_blend_u8.argtypes = [C.POINTER(vp), C.POINTER(i32), i32, i32, i32, i32, i32, vp, i32, i32, i32, vp]
 
     def build_info(self) -> str:
         return self.dll.gimmvfi_build_info().decode()

@@ -755,6 +755,20 @@ int gimmvfi_op_scene_sums(const uint8_t* a, const uint8_t* b, int n, int h, int 
     scene_sums(cx, a, b, n, h, w, sums);
   })
 }
+int gimmvfi_op_blend_u8(const void* const* src, const int* is_f32, int n, int H, int W, int pad_top, int pad_left, uint8_t* dst, int h, int w,
+                        int bgr, void* stream) {
+  gimmvfi_engine* e = nullptr;
+  GV_TRY(e, {
+    if (n < 1 || n > kBlendMax) throw std::runtime_error("blend_u8: n must be in [1, 63]");
+    if (!src || !is_f32 || !dst) throw std::runtime_error("blend_u8: src, is_f32 and dst are required");
+    for (int i = 0; i < n; ++i) if (!src[i]) throw std::runtime_error("blend_u8: a source pointer is null");
+    if (h < 1 || w < 1 || pad_top < 0 || pad_left < 0 || pad_top + h > H || pad_left + w > W)
+      throw std::runtime_error("blend_u8: the crop (pad_top, pad_left, h, w) must lie inside the H x W rows");
+    if ((int64_t)H * W >= ((int64_t)1 << 31)) throw std::runtime_error("blend_u8: H * W must be below 2^31");
+    Ctx cx = op_ctx(stream);
+    blend_u8(cx, src, is_f32, n, H, W, pad_top, pad_left, dst, h, w, bgr);
+  })
+}
 int gimmvfi_op_pixel_shuffle(const gimmvfi_view* src, const gimmvfi_view* dst, int times, void* stream) {
   gimmvfi_engine* e = nullptr;
   GV_TRY(e, { Ctx cx = op_ctx(stream); pixel_shuffle(cx, to_tv(src), to_tv(dst), times); })

@@ -453,6 +453,11 @@ void flow_to_image(Ctx& cx, const FlowView& flow, int has_clip, float clip, int 
 // scene-cut sums of n frame pairs: a, b (n,h,w,3) uint8 RGB, pair i = (a[i], b[i]) -> sums[i] = (sum |dH|, sum |dS|, sum |dV|) of
 // their 8-bit HSV (cv2.COLOR_RGB2HSV); every sum written, bit-exact on every run
 void scene_sums(Ctx& cx, const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums);
+// one output frame of a shutter blend: dst (h,w,3) uint8 = trunc(clamp(mean of the n sources, 0, 255)), BGR when bgr.  Source i is a
+// float32 (3,H,W) row cropped at (pad_top, pad_left), values x * 255 (is_f32[i]), or an (h,w,3) uint8 RGB frame; one launch
+constexpr int kBlendMax = 63;
+void blend_u8(Ctx& cx, const void* const* src, const int* is_f32, int n, int H, int W, int pad_top, int pad_left, uint8_t* dst, int h, int w,
+              int bgr);
 // forward_interpolate (raft/utils/utils.py:33-63) of n dense (2,h,w) flows -> out (n,2,h,w), which must not overlap flow
 void forward_interpolate(Ctx& cx, const float* flow, int n, int h, int w, float* out);
 void pad_image4(Ctx& cx, const TV& src /*c=3, ld=4*/, const TV& dst /*h+2p, w+2p, ld 4*/, int pad);

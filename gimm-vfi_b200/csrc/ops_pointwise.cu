@@ -1883,4 +1883,130 @@ void scene_sums(Ctx& cx, const uint8_t* a, const uint8_t* b, int n, int h, int w
 #endif
 }
 
+// ---- shutter blend: one output frame as the mean of its sub-frames (FrameRateConverter's shutter_angle) ----
+// The per-pixel arithmetic, shared by the kernel and the host simulation: a channel's float32 sum over the sources in order,
+// acc = acc + v with v = x * 255 for a float source and the byte for a uint8 one, then trunc(clamp(acc / n, 0, 255)).  Every operation
+// is rounded once (no contraction into an FMA), so n = 1 is pred_to_u8's (x * 255).astype(uint8), and n copies of one byte sum to an
+// exact integer that divides back to that byte.
+GV_HD float blend_add(float acc, float x, bool f32) { return fv_add(acc, f32 ? fv_mul(x, 255.f) : x); }
+GV_HD uint8_t blend_byte(float acc, int n) {
+  float v = fv_div(acc, (float)n);
+  v = v < 0.f ? 0.f : (v > 255.f ? 255.f : v);
+  return (uint8_t)v;
+}
+struct BlendArgs {
+  const void* src[kBlendMax];
+  uint64_t f32;   // bit i: source i is a float32 (3,H,W) row, read through the crop; otherwise an (h,w,3) uint8 RGB frame
+  uint64_t vec;   // bit i: uint8 source i starts on a 16-byte boundary; bit 63: so does dst
+  uint8_t* dst; int n, h, w, H, W, pt, pl, bgr;
+};
+// host simulation: one item per output byte
+struct BlendU8K {
+  BlendArgs a;
+  GV_HD void operator()(int64_t i) const {
+    const int c = (int)(i % 3); const int64_t p = i / 3;
+    const int cs = a.bgr ? 2 - c : c;
+    const int64_t fo = ((int64_t)cs * a.H + p / a.w + a.pt) * a.W + p % a.w + a.pl;
+    float acc = 0.f;
+    for (int k = 0; k < a.n; ++k) {
+      const bool f = (a.f32 >> k) & 1;
+      acc = blend_add(acc, f ? static_cast<const float*>(a.src[k])[fo] : (float)static_cast<const uint8_t*>(a.src[k])[p * 3 + cs], f);
+    }
+    a.dst[i] = blend_byte(acc, a.n);
+  }
+};
+#ifndef GV_HOSTSIM
+constexpr int kBlendThreads = 256, kBlendPerThread = 4;
+constexpr int kBlendTile = kBlendThreads * kBlendPerThread;   // pixels per CTA tile: 3072 bytes of a uint8 frame, 192 16-byte words
+// `bytes` bytes of a uint8 frame into the tile in shared memory (16-byte words where `vec`, the tail byte by byte), and back out
+__device__ __forceinline__ void blend_tile_load(uint8_t* tile, const uint8_t* src, int bytes, bool vec) {
+  const int words = vec ? bytes / 16 : 0;
+  for (int k = threadIdx.x; k < words; k += kBlendThreads) reinterpret_cast<uint4*>(tile)[k] = __ldcs(reinterpret_cast<const uint4*>(src) + k);
+  for (int k = words * 16 + threadIdx.x; k < bytes; k += kBlendThreads) tile[k] = __ldcs(src + k);
+}
+__device__ __forceinline__ void blend_tile_store(uint8_t* dst, const uint8_t* tile, int bytes, bool vec) {
+  const int words = vec ? bytes / 16 : 0;
+  for (int k = threadIdx.x; k < words; k += kBlendThreads) reinterpret_cast<uint4*>(dst)[k] = reinterpret_cast<const uint4*>(tile)[k];
+  for (int k = words * 16 + threadIdx.x; k < bytes; k += kBlendThreads) dst[k] = tile[k];
+}
+// A CTA takes tiles of kBlendTile consecutive output pixels; thread x holds pixels x, x + 256, ... of a tile, so a float source is read
+// with lanes along x, and a uint8 source goes through shared memory in 16-byte words.  The output is assembled in shared memory and
+// stored the same way.  Each source byte is read once (.cs: a sub-frame is not read again).
+__global__ void __launch_bounds__(kBlendThreads) blend_u8_kernel(const __grid_constant__ BlendArgs a) {
+  __shared__ uint4 words[kBlendTile * 3 / 16];
+  uint8_t* tile = reinterpret_cast<uint8_t*>(words);
+  const int64_t P = (int64_t)a.h * a.w, plane = (int64_t)a.H * a.W;
+  for (int64_t t0 = (int64_t)blockIdx.x * kBlendTile; t0 < P; t0 += (int64_t)gridDim.x * kBlendTile) {
+    const int cnt = P - t0 < kBlendTile ? (int)(P - t0) : kBlendTile;
+    int64_t fo[kBlendPerThread];
+    float acc[kBlendPerThread][3];
+#pragma unroll
+    for (int q = 0; q < kBlendPerThread; ++q) {
+      const int64_t p = t0 + q * kBlendThreads + threadIdx.x;
+      fo[q] = (p / a.w + a.pt) * a.W + p % a.w + a.pl;
+      acc[q][0] = acc[q][1] = acc[q][2] = 0.f;
+    }
+    for (int i = 0; i < a.n; ++i) {
+      if ((a.f32 >> i) & 1) {
+        const float* s = static_cast<const float*>(a.src[i]);
+        float v[kBlendPerThread][3];
+#pragma unroll
+        for (int q = 0; q < kBlendPerThread; ++q)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) v[q][c] = q * kBlendThreads + (int)threadIdx.x < cnt ? __ldcs(s + c * plane + fo[q]) : 0.f;
+#pragma unroll
+        for (int q = 0; q < kBlendPerThread; ++q)
+#pragma unroll
+          for (int c = 0; c < 3; ++c) acc[q][c] = blend_add(acc[q][c], v[q][c], true);
+      } else {
+        __syncthreads();   // the tile's last contents are consumed
+        blend_tile_load(tile, static_cast<const uint8_t*>(a.src[i]) + t0 * 3, cnt * 3, (a.vec >> i) & 1);
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < kBlendPerThread; ++q) {
+          const int j = q * kBlendThreads + threadIdx.x;
+          if (j < cnt)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) acc[q][c] = blend_add(acc[q][c], (float)tile[j * 3 + c], false);
+        }
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < kBlendPerThread; ++q) {
+      const int j = q * kBlendThreads + threadIdx.x;
+      if (j < cnt)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) tile[j * 3 + c] = blend_byte(a.bgr ? acc[q][2 - c] : acc[q][c], a.n);   // (constant indices: registers)
+    }
+    __syncthreads();
+    blend_tile_store(a.dst + t0 * 3, tile, cnt * 3, (a.vec >> 63) & 1);
+  }
+}
+#endif
+void blend_u8(Ctx& cx, const void* const* src, const int* is_f32, int n, int H, int W, int pad_top, int pad_left, uint8_t* dst, int h, int w,
+              int bgr) {
+  if (cx.dry) return;
+  BlendArgs a{};
+  int floats = 0;
+  for (int i = 0; i < n; ++i) {
+    a.src[i] = src[i];
+    if (is_f32[i]) { a.f32 |= 1ull << i; ++floats; }
+    else if (aligned(src[i], 16)) a.vec |= 1ull << i;
+  }
+  if (aligned(dst, 16)) a.vec |= 1ull << 63;
+  a.dst = dst; a.n = n; a.h = h; a.w = w; a.H = H; a.W = W; a.pt = pad_top; a.pl = pad_left; a.bgr = bgr;
+  const int64_t P = (int64_t)h * w;
+#ifdef GV_HOSTSIM
+  parallel_for(cx, P * 3, BlendU8K{a}, "blend_u8");
+#else
+  cx.launches++;
+  if (cx.prof) cx.prof->begin(cx.stream, "blend_u8", (double)P * (3.0 + 12.0 * floats + 3.0 * (n - floats)));
+  const int64_t blocks = std::min((P + kBlendTile - 1) / kBlendTile, (int64_t)cx.sm_count * 8);
+  blend_u8_kernel<<<(unsigned)blocks, kBlendThreads, 0, cx.stream>>>(a);
+  gv_check_launch("blend_u8");
+  if (cx.prof) cx.prof->end(cx.stream);
+#endif
+}
+
 }  // namespace gv

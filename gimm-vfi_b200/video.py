@@ -116,6 +116,7 @@ class _Cuts:
 
     def reset(self):
         self.cuts, self._cut, self._waiting, self._hw = [], set(), [], None
+        self.decided = 0   # every pair (j - 1, j) with j <= decided has been read back
 
     def push(self, j: int, prev_u8: torch.Tensor, cur_u8: torch.Tensor):
         self._waiting.append((j, _pair_sums(prev_u8, cur_u8)))
@@ -129,6 +130,7 @@ class _Cuts:
             if s >= self.threshold:
                 self.cuts.append(j)
                 self._cut.add(j)
+        self.decided = self._waiting[-1][0]
         self._waiting = []
 
     def __contains__(self, j: int) -> bool:
@@ -138,6 +140,32 @@ class _Cuts:
 def _as_output(u8: torch.Tensor, bgr: bool) -> torch.Tensor:
     """an input frame as an output frame: its bytes, BGR-flipped when `bgr`"""
     return u8.flip(-1) if bgr else u8.clone()
+
+
+def blend_u8(sources: List[torch.Tensor], padder: InputPadder, bgr: bool = True) -> torch.Tensor:
+    """gimmvfi_op_blend_u8: one (h,w,3) uint8 output frame as the mean of 1 to 63 sources on one device, each a padded (3,H,W) float32
+    engine prediction (value x * 255, cropped with the padder's unpad box) or an (h,w,3) uint8 RGB frame (value its byte), both
+    contiguous.  Each channel is the float32 sum over the sources in order, then trunc(clamp(sum / n, 0, 255)): one source gives
+    unpad_u8's bytes, and n copies of one frame give that frame.  BGR when `bgr`.  One launch."""
+    n = len(sources)
+    if not 1 <= n <= 63:
+        raise ValueError("blend_u8: 1 to 63 sources, got %d" % n)
+    h, w = padder.ht, padder.wd
+    H, W = padder.padded_shape
+    top, _, left, _ = padder.unpad_box(H, W)
+    dev = sources[0].device
+    for s in sources:
+        shape = (3, H, W) if s.dtype == torch.float32 else (h, w, 3)
+        if s.dtype not in (torch.float32, torch.uint8) or tuple(s.shape) != shape or not s.is_contiguous() or s.device != dev:
+            raise ValueError("blend_u8: a source must be a contiguous (3,%d,%d) float32 or (%d,%d,3) uint8 tensor on %s, got %s %s"
+                             % (H, W, h, w, dev, tuple(s.shape), s.dtype))
+    out = torch.empty(h, w, 3, dtype=torch.uint8, device=dev)
+    ptrs = (C.c_void_p * n)(*[s.data_ptr() for s in sources])
+    kinds = (C.c_int * n)(*[int(s.dtype == torch.float32) for s in sources])
+    lib = default_lib()
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream) if dev.type == "cuda" else None
+    lib.check(lib.dll.gimmvfi_op_blend_u8(ptrs, kinds, n, H, W, top, left, C.c_void_p(out.data_ptr()), h, w, int(bgr), stream))
+    return out
 
 
 def flow_images(padder: InputPadder, flowt: List[torch.Tensor], bgr: bool) -> List[torch.Tensor]:
@@ -185,14 +213,41 @@ def interpolate_pair_u8(model, frame0_u8: torch.Tensor, frame1_u8: torch.Tensor,
     return (frames, flow_images(padder, out["flowt"], bgr)) if with_flow else frames
 
 
+class _Sample:
+    """one instant of an output: input frame f (u8: our uint8 copy of it, None without copies), or the interpolation of pair (j - 1, j) at
+    t, which falls back to frame f, the nearer one (offset <= 1/2: the earlier), if the pair turns out to be a scene cut.  After the engine
+    call, `out` holds what it made of the instant (the output frame, or with a shutter the padded float prediction) and `flow` its flowt."""
+
+    __slots__ = ("pair", "t", "f", "u8", "out", "flow")
+
+    def __init__(self, pair, t, f: int, u8: Optional[torch.Tensor]):
+        self.pair, self.t, self.f, self.u8, self.out, self.flow = pair, t, f, u8, None, None
+
+
+class _Entry:
+    """one output frame in the queue: its samples in time order, `own` the one at the output's own instant.  Only a shutter's outputs
+    have more than one sample: `pending` holds the instants of the window not placed yet (after the last frame pushed), `needs` the last
+    j whose pair (j - 1, j) must be decided (scene score read back) before the output's shot is known, `tau` its own instant."""
+
+    __slots__ = ("samples", "own", "pending", "needs", "tau")
+
+    def __init__(self, samples=(), pending=(), needs: int = 0, tau=None):
+        self.samples, self.pending, self.needs, self.tau = list(samples), list(pending), needs, tau
+        self.own = self.samples[0] if len(self.samples) == 1 else None
+
+
 class _Stream:
-    """What VideoInterpolator and FrameRateConverter share: a clip's input frames, pushed one by one, become a stream of outputs.  Pushing
-    input frame j schedules the output instants in (j - 1, j] (the subclass's _instants).  An output is an input frame passed through, or
-    the interpolation of the pair (j - 1, j) at some t, which falls back to the nearer input frame (offset <= 1/2: the earlier) if the
-    pair turns out to be a scene cut.  The outputs wait in a queue in output order.  A push that leaves no interpolation waiting returns
-    the queue and reads nothing back.  A push that brings the distinct pairs waiting to pairs_per_call, and flush(), read every waiting
-    scene score in one copy, turn the entries of cut pairs into their fallback frames, and send the pairs left to one engine call (the
-    subclass's _run) on only the frames they use; then the whole queue comes back in order."""
+    """What VideoInterpolator and FrameRateConverter share: a clip's input frames, pushed one by one, become a stream of outputs.  An
+    output is a queue entry holding one sample, or with FrameRateConverter's shutter the samples of its exposure window.  Pushing input
+    frame j places the instants in (j - 1, j] (the subclass's _schedule): a sample is an input frame passed through, or the interpolation
+    of the pair (j - 1, j) at some t, which falls back to the nearer input frame (offset <= 1/2: the earlier) if the pair turns out to be a
+    scene cut.  The outputs wait in a queue in output order.  A push that leaves no interpolation waiting returns the complete outputs at
+    the head of the queue and reads nothing back, unless the head waits only for scene scores (a shutter window of input frames alone):
+    then it reads them back in one copy.  A push that brings the distinct pairs waiting to pairs_per_call, and flush(), read every
+    waiting scene score in one copy, turn the samples of cut pairs into their fallback frames, and send the pairs left to one engine call
+    (the subclass's _run) on only the frames they use; then the complete outputs come back in order.  An output is complete when each of
+    its samples is placed and made, and the pairs its window spans are decided; without a shutter that is every output after a call.  An
+    output still waiting after a call keeps copies of its sub-frames, so what waits is at most a few frames per output."""
 
     with_flow = False
     _passes_frames = False   # whether an output instant can fall on an input frame (then uint8 copies are always kept)
@@ -213,11 +268,10 @@ class _Stream:
     def reset(self):
         """start a new clip: the next frame pushed is input frame 0"""
         self._n = 0             # input frames pushed
-        # the scheduled outputs, in order: ((j - 1, j), t, fallback) for an interpolation, (None, None, frame) for an input frame, the
-        # frames being our uint8 copies (None without copies)
-        self._queue = []
+        self._queue = []        # the scheduled outputs (_Entry), in order
         self._padded = {}       # input index -> padded float frame (3,H,W): the frames of the pairs waiting, and the last frame
         self._last_u8 = None    # the copy of the last frame pushed
+        self._ended = False     # flush() ended the clip: the next push starts a new one
         if self._scene is not None:
             self._scene.reset()
 
@@ -229,11 +283,13 @@ class _Stream:
     @torch.no_grad()
     def flush(self):
         """interpolate what is waiting and return every output scheduled, in order, as push() does; nothing is left waiting"""
-        return self._emit(True)
+        return self._emit(True, final=True)
 
     @torch.no_grad()
     def push(self, frame_u8: torch.Tensor):
         """the next input frame, (h,w,3) uint8 RGB on the device -> the outputs completed by it, in order (uint8 (h,w,3), BGR when `bgr`)"""
+        if self._ended:
+            self.reset()
         if self._padder is None or (self._padder.ht, self._padder.wd) != tuple(frame_u8.shape[:2]):
             if self._queue:
                 raise ValueError("%s: the frame size changed with outputs still waiting; flush() first" % type(self).__name__)
@@ -246,45 +302,83 @@ class _Stream:
             self._scene.push(j, prev_u8, cur_u8)
         if cur_u8 is None:   # the padded frame is then the only copy of frame j that the next pair can use
             self._padded[j] = self._padder.pad_u8(frame_u8.unsqueeze(0))[0]
-        for off, t in self._instants(j):
-            fallback = prev_u8 if off <= Fraction(1, 2) else cur_u8
-            if t is None:
-                self._queue.append((None, None, fallback))
-                continue
-            for f, u8 in ((j - 1, prev_u8), (j, frame_u8)):
-                if f not in self._padded:
-                    self._padded[f] = self._padder.pad_u8(u8.unsqueeze(0))[0]
-            self._queue.append(((j - 1, j), t, fallback))
+        self._schedule(j, prev_u8, frame_u8, cur_u8)
         self._last_u8 = cur_u8
-        waiting = {pair for pair, _, _ in self._queue if pair is not None}
+        waiting = {s.pair for e in self._queue for s in e.samples if s.pair is not None and s.out is None}
         if waiting and len(waiting) < self.pairs_per_call:
             return ([], []) if self.with_flow else []
-        return self._emit(bool(waiting))
+        # an output whose samples are all placed and made may still wait for the scores of the pairs its window spans (a shutter whose
+        # samples all fall on input frames makes no engine call): read them back now rather than at the next call
+        head = self._queue[0] if self._queue else None
+        blocked = self._scene is not None and head is not None and not head.pending and head.needs > self._scene.decided
+        return self._emit(bool(waiting) or blocked)
 
-    def _emit(self, decide: bool):
-        """every output in the queue, in order, leaving it empty.  decide: read the waiting scene scores first and turn the entries of
-        cut pairs into their fallback frames.  An engine call that raises drops the outputs it was to make, and the clip goes on with the
-        next frame pushed."""
+    def _schedule(self, j: int, prev_u8, frame_u8, cur_u8):
+        """queue one output per instant of the subclass's _instants(j)"""
+        for off, t in self._instants(j):
+            self._queue.append(_Entry([self._sample(j, off, t, prev_u8, frame_u8, cur_u8)]))
+
+    def _sample(self, j: int, off: Fraction, t: Optional[float], prev_u8, frame_u8, cur_u8) -> _Sample:
+        """the sample at offset off in (0, 1] into (j - 1, j]: an input frame when t is None, else the query (j - 1, j, t)"""
+        f, u8 = (j - 1, prev_u8) if off <= Fraction(1, 2) else (j, cur_u8)
+        if t is None:
+            return _Sample(None, None, f, u8)
+        for g, x in ((j - 1, prev_u8), (j, frame_u8)):
+            if g not in self._padded:
+                self._padded[g] = self._padder.pad_u8(x.unsqueeze(0))[0]
+        return _Sample((j - 1, j), t, f, u8)
+
+    def _emit(self, decide: bool, final: bool = False):
+        """the complete outputs at the head of the queue, in order (final: every output).  decide: read the waiting scene scores first and
+        turn the samples of cut pairs into their fallback frames.  An engine call that raises drops the outputs waiting, and the clip goes
+        on with the next frame pushed."""
         if decide and self._scene is not None:
             self._scene.resolve()
-            self._queue = [(None, None, u8) if pair is not None and pair[1] in self._scene else (pair, t, u8) for pair, t, u8 in self._queue]
+            for e in self._queue:
+                for s in e.samples:
+                    if s.pair is not None and s.pair[1] in self._scene:
+                        s.pair = s.t = None
+        if final:
+            self._end_clip()
         queue, self._queue = self._queue, []
-        interp = [(pair, t) for pair, t, _ in queue if pair is not None]
-        preds = flows = iter(())
+        interp = [s for e in queue for s in e.samples if s.pair is not None and s.out is None]
         if interp:
-            used = sorted({f for pair, _ in interp for f in pair})   # without a cut: every frame since the last call
+            used = sorted({f for s in interp for f in s.pair})   # without a cut: every frame since the last call
             local = {f: i for i, f in enumerate(used)}
-            ims, fl = self._run(used, [self._padded[f] for f in used], [(local[a], local[b], t) for (a, b), t in interp])
-            preds, flows = iter(self._padder.unpad_u8(ims, self.bgr).unbind(0)), iter(fl or ())
+            ims, fl = self._run(used, [self._padded[f] for f in used], [(local[s.pair[0]], local[s.pair[1]], s.t) for s in interp])
+            for s, x in zip(interp, self._preds(ims)):
+                s.out = x
+            for s, x in zip(interp, fl or ()):
+                s.flow = x
         self._padded = {f: x for f, x in self._padded.items() if f == self._n - 1}
-        frames = [next(preds) if pair is not None else _as_output(u8, self.bgr) for pair, _, u8 in queue]
+        decided = self._n - 1 if self._scene is None else self._scene.decided
+        n = len(queue) if final else next((i for i, e in enumerate(queue) if e.pending or e.needs > decided), len(queue))
+        done, self._queue = queue[:n], queue[n:]
+        made = set(interp)
+        for e in self._queue:   # an output still waiting keeps copies of its sub-frames, not the whole output of this call
+            for s in e.samples:
+                if s in made:
+                    s.out = s.out.clone()
+        frames = [self._output(e) for e in done]
         if not self.with_flow:
             return frames
         zero = None
-        if len(interp) < len(queue):   # a cut's pictures are those of a zero flow at the network resolution
-            zero = torch.zeros(2, *self._net_size(*self._padder.padded_shape), dtype=torch.float32, device=queue[0][2].device)
-        pics = [next(flows) if pair is not None else zero for pair, _, _ in queue]
+        if len(interp) < len(done):   # a cut's pictures are those of a zero flow at the network resolution
+            zero = torch.zeros(2, *self._net_size(*self._padder.padded_shape), dtype=torch.float32, device=done[0].own.u8.device)
+        pics = [e.own.flow if e.own.flow is not None else zero for e in done]
         return frames, (flow_images(self._padder, pics, self.bgr) if pics else [])
+
+    def _end_clip(self):
+        """flush(): the last input frame is known"""
+
+    def _preds(self, ims: torch.Tensor):
+        """the engine's predictions (n,3,H,W), in sample order -> what the samples keep: here their uint8 output frames"""
+        return self._padder.unpad_u8(ims, self.bgr).unbind(0)
+
+    def _output(self, e: _Entry) -> torch.Tensor:
+        """a complete entry's output frame"""
+        s = e.own
+        return s.out if s.out is not None else _as_output(s.u8, self.bgr)
 
 
 class VideoInterpolator(_Stream):
@@ -372,6 +466,27 @@ def _rate(x, name: str) -> Fraction:
 SNAP = Fraction(1, 10 ** 6)   # output instants this close to an input frame (in input frames) are that frame
 
 
+def _shutter_angle(x) -> Optional[Fraction]:
+    """None, or a shutter angle in degrees in (0, 360] as an exact rational (floats via their repr, as _rate reads them)"""
+    if x is None:
+        return None
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise ValueError("shutter_angle must be None or a number in (0, 360], got %r" % (x,))
+    try:
+        a = Fraction(x) if isinstance(x, numbers.Rational) else Fraction(repr(float(x)))
+    except (ValueError, OverflowError):
+        raise ValueError("shutter_angle must be None or a number in (0, 360], got %r" % (x,))
+    if not 0 < a <= 360:
+        raise ValueError("shutter_angle must be None or a number in (0, 360], got %r" % (x,))
+    return a
+
+
+def _shutter_samples(x) -> int:
+    if isinstance(x, bool) or not isinstance(x, numbers.Integral) or not 1 <= x <= 63 or x % 2 == 0:
+        raise ValueError("shutter_samples must be an odd int in [1, 63], got %r" % (x,))
+    return int(x)
+
+
 class FrameRateConverter(_Stream):
     """Frame-rate conversion of a clip streamed frame by frame: push() the (h,w,3) uint8 RGB input frames, get the output frames at
     fps_out.  Output frame k shows input time tau_k = k * fps_in / fps_out (in input frames, exact rationals: no drift), for every k with
@@ -391,28 +506,103 @@ class FrameRateConverter(_Stream):
     the engine.  An output instant at offset t into a cut interval is the nearer input frame, the earlier one for t <= 1/2 (its bytes,
     BGR-flipped when `bgr`).  The score of (j - 1, j) is computed on the device when frame j is pushed; the scores are read back once per
     engine call or flush(), when the K pairs with queries of a call are decided, and a call whose pairs are all cuts is not made.
-    `cuts` lists the input indices j whose pair (j - 1, j) scored >= T since the last reset()."""
+    `cuts` lists the input indices j whose pair (j - 1, j) scored >= T since the last reset().
+
+    shutter_angle A (None: off), shutter_samples S (odd, 1 .. 63; default 7): motion blur, as a camera whose shutter is open for A / 360 of
+    each output frame.  Output k's exposure window is w = (A / 360) * fps_in / fps_out input frames wide, centred on tau_k, and its samples
+    are the midpoints of S equal parts of it, s_i = tau_k - w / 2 + (i + 1/2) w / S (exact rationals).  A <= 360 keeps windows apart, so no
+    two outputs share an instant.  Each sample takes the rule of an output instant above (an input frame within SNAP, a query, the nearer
+    frame in a cut pair).  A sample before frame 0 or after the last frame is dropped, and so is one whose frame or pair lies in another
+    shot than the output's own (a shot: the frames between two cuts).  The output's own shot is that of tau_k, the middle sample, which is
+    why S is odd: that sample is never dropped, and it is the instant the converter shows without a shutter.  With an even S and a wide
+    window every sample could land in another shot (120 -> 24 at 360 degrees with S = 2 around a one-frame shot).  The output is the mean of
+    the n samples kept, each channel trunc(clamp(sum / n, 0, 255)) of the float32 sum in sample order of x * 255 (an engine frame) or the
+    byte (an input frame): gimmvfi_op_blend_u8 (blend_u8), one launch per output frame.  S = 1 gives the bytes of shutter_angle=None for
+    a clip ended by one flush(); unlike the converter without a shutter, a shutter's flush() always ends the clip (below).
+    Averaging is in the frames' encoded values, as ffmpeg's tmix does; the window adds to the blur the input already has.  A pair still goes
+    to exactly one engine call, with every sample any output places in it: pushing frame j places every sample in (j - 1, j], including
+    those of outputs whose tau_k lies up to w / 2 after frame j, and an output comes back once each pair its window spans is decided and
+    interpolated (the push that completes a window of input frames alone reads its scene scores back itself).  The sub-frames of an output are kept until it is complete, so its bytes do not depend on K.  flush() ends the clip:
+    samples after the last frame are dropped, so the windows that cross the end are cut short and the clip cannot go on; the next push()
+    starts a new clip (input frame 0, `cuts` cleared).  Without a shutter, flush() leaves the clip open, as it always has.  The samples of
+    an output past the end of the clip (at most one output's) may have been interpolated by then and are thrown away."""
 
     _passes_frames = True
 
     def __init__(self, model, fps_in, fps_out, ds_factor: Optional[float] = None, bgr: bool = True, pairs_per_call: int = 1,
-                 scene_threshold: Optional[float] = None):
+                 scene_threshold: Optional[float] = None, shutter_angle=None, shutter_samples: int = 7):
         if isinstance(pairs_per_call, bool) or int(pairs_per_call) < 1:
             raise ValueError("pairs_per_call must be >= 1, got %r" % (pairs_per_call,))
+        self.shutter_angle, self.shutter_samples = _shutter_angle(shutter_angle), _shutter_samples(shutter_samples)
         super().__init__(model, ds_factor, bgr, pairs_per_call, scene_threshold)
         self.fps_in, self.fps_out = _rate(fps_in, "fps_in"), _rate(fps_out, "fps_out")
         self.step = self.fps_in / self.fps_out   # input frames per output frame
+        # the exposure window in input frames (None: no shutter)
+        self.window = None if self.shutter_angle is None else self.shutter_angle / 360 * self.step
 
     def reset(self):
         super().reset()
         self._k = 0             # next output index to schedule
 
+    @staticmethod
+    def _instant(j: int, x: Fraction):
+        """an instant x in (j - 1, j] -> (its offset in (0, 1], the float32 t of its query or None for an input frame)"""
+        off = x - (j - 1)
+        # input frame j, or (a hair after it) frame j - 1; any other instant is interpolated at the float32 t the engine receives
+        return off, None if off >= 1 - SNAP or off <= SNAP else float(np.float32(float(off)))
+
     def _instants(self, j: int):
         while self._k * self.step <= j:   # the output instants in (j - 1, j] (frame 0: the instant 0)
-            off = self._k * self.step - (j - 1)   # in (0, 1]
+            x = self._k * self.step
             self._k += 1
-            # input frame j, or (a hair after it) frame j - 1; any other instant is interpolated at the float32 t the engine receives
-            yield off, None if off >= 1 - SNAP or off <= SNAP else float(np.float32(float(off)))
+            yield self._instant(j, x)
+
+    def _schedule(self, j: int, prev_u8, frame_u8, cur_u8):
+        if self.window is None:
+            return super()._schedule(j, prev_u8, frame_u8, cur_u8)
+        w, S = self.window, self.shutter_samples
+        # every output whose window starts by frame j, so that each sample in (j - 1, j] is placed now
+        while self._k * self.step - w / 2 + w / (2 * S) <= j:
+            tau = self._k * self.step
+            inst = [tau - w / 2 + (2 * i + 1) * w / (2 * S) for i in range(S)]
+            self._queue.append(_Entry(pending=inst, needs=math.ceil(inst[-1]) if S > 1 else 0, tau=tau))
+            self._k += 1
+        for e in self._queue:
+            while e.pending and e.pending[0] <= j:
+                x = e.pending.pop(0)
+                if x < 0:   # before frame 0
+                    continue
+                s = self._sample(j, *self._instant(j, x), prev_u8, frame_u8, cur_u8)
+                e.samples.append(s)
+                if x == e.tau:
+                    e.own = s
+
+    def _end_clip(self):
+        if self.window is None:
+            return
+        last = self._n - 1
+        self._queue = [e for e in self._queue if e.tau <= last]
+        for e in self._queue:
+            e.pending = []    # the samples after the last frame
+        self._ended = True
+
+    def _preds(self, ims: torch.Tensor):
+        if self.window is None:
+            return super()._preds(ims)
+        return ims.contiguous().unbind(0)   # the sub-frames stay padded float until their outputs are blended
+
+    def _kept(self, e: _Entry) -> List[_Sample]:
+        """the samples of a complete entry in its own shot: no cut between a sample's frame (a pair: its first frame) and the own one's"""
+        if self._scene is None or len(e.samples) == 1:
+            return e.samples
+        pos = lambda s: s.f if s.pair is None else s.pair[0]
+        own = pos(e.own)
+        return [s for s in e.samples if not any(c in self._scene for c in range(min(pos(s), own) + 1, max(pos(s), own) + 1))]
+
+    def _output(self, e: _Entry) -> torch.Tensor:
+        if self.window is None:
+            return super()._output(e)
+        return blend_u8([s.out if s.pair is not None else s.u8 for s in self._kept(e)], self._padder, self.bgr)
 
     def _run(self, used, frames, queries):
         return self.model._interpolate_at(torch.stack(frames, 0), queries, self.ds, False)["imgt_pred"], None

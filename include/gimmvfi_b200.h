@@ -476,6 +476,14 @@ int gimmvfi_op_forward_interpolate(const float* flow, int n, int h, int w, float
  * Every sum is written (the op zeroes what it accumulates into).  Integer sums: bit-exact on every run.  The score is
  * (sums[i][0] + sums[i][1] + sums[i][2]) / (3 h w).  Refuses n < 0, h or w < 1 and h*w >= 2^31. */
 int gimmvfi_op_scene_sums(const uint8_t* a, const uint8_t* b, int n, int h, int w, uint64_t* sums, void* stream);
+/* One output frame of a shutter blend (motion blur): dst (h,w,3) uint8, contiguous, on the device, is the mean of n sources, 1 <= n <= 63.
+ * Source i is src[i], on the device: with is_f32[i] != 0, one (3,H,W) float32 row of an engine output (imgt_pred), read through the crop
+ * rows pad_top .. pad_top+h-1 and columns pad_left .. pad_left+w-1, value x * 255; otherwise a contiguous (h,w,3) uint8 RGB frame, value
+ * its byte.  Each channel is acc = acc + v over the sources in order in float32, then trunc(clamp(acc / n, 0, 255)), each operation rounded
+ * once: n = 1 gives gimmvfi_op_pred_to_u8's bytes, and n copies of one uint8 frame give that frame.  bgr != 0 writes BGR.  One launch, no
+ * allocation.  Refuses n outside [1, 63], a null pointer, h or w < 1, a crop outside H x W and H*W >= 2^31. */
+int gimmvfi_op_blend_u8(const void* const* src, const int* is_f32, int n, int H, int W, int pad_top, int pad_left, uint8_t* dst, int h, int w,
+                        int bgr, void* stream);
 /* nn.PixelShuffle(2) applied `times` times */
 int gimmvfi_op_pixel_shuffle(const gimmvfi_view* src, const gimmvfi_view* dst, int times, void* stream);
 
